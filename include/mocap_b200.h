@@ -273,14 +273,38 @@ MOCAP_API int  mocap_bundle_adjust_host(mocap_ctx* ctx, const double* obs, const
 MOCAP_API int  mocap_bundle_adjust_dev(mocap_ctx* ctx, const double* obs, const uint8_t* mask, int n_points_max,
                              const int32_t* n_points, double* R, double* t, const mocap_ba_options* opt,
                              mocap_ba_report* report);
-/* CTAs of k_ba_solve for this context (1 .. number of SMs; 0 = the default, one per SM).  One solve is a cooperative
- * grid whose serial sections (dense solves, tridiagonalisation) leave most CTAs waiting at the grid barrier, so
- * INDEPENDENT solves -- the reference runs one bundle_adjustment per recorded batch (index.py:249-276), a session with
- * several batches has several -- finish sooner side by side: K contexts on K streams with SMs / K CTAs each
- * (measured on an H100 SXM at a 400 W power limit, a config-3 step of S1-S3 over 4000 frame-sets plus 4 solves of 8 cameras
- * x 18 800 points: 13.6 ms with the solves in turn on 132 CTAs, 11.3 ms as 2 x 66, 10.4 ms as 4 x 33).
- * The result does not depend on the number of CTAs. */
+/* CTA budget G of k_ba_solve for this context (1 .. number of SMs; 0 = the default, one per SM).  A single solve
+ * (mocap_bundle_adjust_dev) runs on all G CTAs; a batch of K solves (mocap_bundle_adjust_batch_dev) splits them,
+ * problem k getting G / K + (k < G % K).  One solve is a cooperative grid whose serial sections (dense solves,
+ * tridiagonalisation) leave most CTAs waiting at the grid barrier, so INDEPENDENT solves -- the reference runs one
+ * bundle_adjustment per recorded batch (index.py:249-276), a session with several batches has several -- finish sooner
+ * side by side, in one batched call or as K contexts on K streams with G = SMs / K each (measured on an H100 SXM at a
+ * 400 W power limit, a config-3 step of S1-S3 over 4000 frame-sets plus 4 solves of 8 cameras x 18 800 points:
+ * 13.6 ms with the solves in turn on 132 CTAs, 11.3 ms as 2 x 66, 10.4 ms as 4 x 33 on four contexts).
+ * Results depend on the number of CTAs a solve runs on only in the rounding of its sums, and are reproducible for
+ * a given number. */
 MOCAP_API int  mocap_set_ba_grid(mocap_ctx* ctx, int n_ctas);
+
+/* One problem of a batched bundle adjustment: the arguments of mocap_bundle_adjust_dev that differ per solve.
+ * DEVICE pointers; n_points may be NULL (= n_points_max), report may be NULL. */
+#define MOCAP_BA_MAX_BATCH 16
+typedef struct mocap_ba_problem {
+    const double*    obs;          /* [n_points_max][n_cam][2]                                   */
+    const uint8_t*   mask;         /* [n_points_max][n_cam]                                      */
+    int              n_points_max;
+    const int32_t*   n_points;     /* device int32, read by the kernel                           */
+    double*          R;            /* [n_cam][9] in/out                                          */
+    double*          t;            /* [n_cam][3] in/out                                          */
+    mocap_ba_report* report;
+} mocap_ba_problem;
+/* n_problems (1 .. MOCAP_BA_MAX_BATCH, and at most the context's CTA budget, mocap_set_ba_grid) INDEPENDENT bundle
+ * adjustments in ONE cooperative launch on the context's stream; never synchronises.  problems is a HOST array;
+ * every problem uses the context's cameras and the one set of options opt (HOST, NULL = defaults).  Problem k runs
+ * on its own G / K + (k < G % K) CTAs with its own barrier and workspace, and gives the same bits (poses and report,
+ * phase_ms aside) as mocap_bundle_adjust_dev on a context whose budget is that number of CTAs; a problem without a
+ * point that has two views reports status -3 and keeps its poses, the others are unaffected. */
+MOCAP_API int  mocap_bundle_adjust_batch_dev(mocap_ctx* ctx, const mocap_ba_problem* problems, int n_problems,
+                                   const mocap_ba_options* opt);
 /* Matcher output of a batch -> the explicit correspondences S4 consumes (BASELINE config 3: S1-S3, then one
  * bundle adjustment per batch), on the device: track_xy int32 [n_frame_sets][max_roots][n_cam][2] as written by
  * mocap_pipeline_tracks_dev ((-1, -1) = no view), n_obj / err the matcher's outputs; tracks whose reprojection

@@ -37,6 +37,13 @@ class BAReport(C.Structure):
                 ("n_tr_newton", C.c_int), ("phase_ms", C.c_float * 8)]
 
 
+class BAProblem(C.Structure):
+    _fields_ = [("obs", C.c_void_p), ("mask", C.c_void_p), ("n_points_max", C.c_int), ("n_points", C.c_void_p),
+                ("R", C.c_void_p), ("t", C.c_void_p), ("report", C.c_void_p)]
+
+
+MOCAP_BA_MAX_BATCH = 16
+
 # every symbol include/mocap_b200.h declares: name -> (restype, argtypes)
 _P = C.c_void_p
 SYMBOLS = {
@@ -65,6 +72,7 @@ SYMBOLS = {
     "mocap_bundle_adjust_host": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, C.POINTER(BAOptions), C.POINTER(BAReport)]),
     "mocap_bundle_adjust_dev": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, _P, C.POINTER(BAOptions), _P]),
     "mocap_set_ba_grid": (C.c_int, [_P, C.c_int]),
+    "mocap_bundle_adjust_batch_dev": (C.c_int, [_P, C.POINTER(BAProblem), C.c_int, C.POINTER(BAOptions)]),
     "mocap_tracks_to_observations_dev": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_double, _P, _P, _P, C.c_int]),
     "mocap_pipeline_tracks_dev": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P]),
     "mocap_ba_residuals_host": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, _P, _P, C.POINTER(C.c_int)]),

@@ -21,7 +21,7 @@ import threading
 import numpy as np
 
 from . import _lib
-from ._lib import MocapError, Config, BAOptions, BAReport, check
+from ._lib import MocapError, Config, BAOptions, BAProblem, BAReport, check
 
 THRESHOLD = 51   # cv.threshold(grey, 255*0.2, 255, THRESH_BINARY) on uint8 == pix > 51 (helpers.py:146)
 
@@ -273,8 +273,10 @@ class MocapContext:
         return out
 
     def set_ba_grid(self, n_ctas=0):
-        """CTAs of the device-resident bundle adjustment of this context (0: one per SM).  Independent solves finish sooner
-        side by side: K contexts on K streams with SMs // K CTAs each (mocap_set_ba_grid, include/mocap_b200.h)."""
+        """CTA budget G of the device-resident bundle adjustment of this context (0: one per SM).  A single solve runs on G
+        CTAs, a batch of K (``bundle_adjust_batch_dev``) splits them, G // K + (k < G % K) for problem k.  Independent
+        solves finish sooner side by side: in one batched call, or as K contexts on K streams with SMs // K CTAs each
+        (mocap_set_ba_grid, include/mocap_b200.h)."""
         self._check(self.lib.mocap_set_ba_grid(self.h, int(n_ctas)))
 
     def bundle_adjust_dev(self, obs, mask, R, t, n_points=None, report=None, ftol=1e-2, max_nfev=0, prefit=True, jacobian=1,
@@ -292,6 +294,30 @@ class MocapContext:
         self._check(self.lib.mocap_bundle_adjust_dev(self.h, _ptr(obs), _ptr(mask), obs.shape[0], _ptr(n_points), _ptr(R), _ptr(t),
                                                      C.byref(opt), _ptr(report)))
         return report
+
+    def bundle_adjust_batch_dev(self, problems, ftol=1e-2, max_nfev=0, prefit=True, jacobian=1, prefit_max_iter=50):
+        """Several independent S4 solves in ONE cooperative launch (mocap_bundle_adjust_batch_dev): problems is a list of
+        dicts with the tensors ``bundle_adjust_dev`` takes -- "obs", "mask", "R", "t" and optionally "n" (int32 cuda [1])
+        and "report" -- sharing this context's cameras and one set of options.  Problem k runs on G // K + (k < G % K) of
+        the context's G CTAs (``set_ba_grid``) and gives the bits ``bundle_adjust_dev`` gives on that many.  No
+        synchronisation.  Returns one report tensor per problem (decode with ``decode_ba_report``)."""
+        torch = _torch()
+        opt = BAOptions()
+        self.lib.mocap_ba_default_options(C.byref(opt))
+        opt.ftol, opt.max_nfev, opt.prefit, opt.jacobian, opt.prefit_max_iter = ftol, max_nfev, 1 if prefit else 0, jacobian, prefit_max_iter
+        reports = []
+        arr = (BAProblem * max(1, len(problems)))()
+        for k, p in enumerate(problems):
+            obs = p.get("obs")
+            rep = p.get("report")
+            if rep is None:
+                rep = torch.zeros((C.sizeof(BAReport),), dtype=torch.uint8, device=f"cuda:{self.cfg.device}")
+            reports.append(rep)
+            arr[k] = BAProblem(_ptr(obs), _ptr(p.get("mask")), 0 if obs is None else int(obs.shape[0]), _ptr(p.get("n")),
+                               _ptr(p.get("R")), _ptr(p.get("t")), _ptr(rep))
+        self.use_current_stream()
+        self._check(self.lib.mocap_bundle_adjust_batch_dev(self.h, arr, len(problems), C.byref(opt)))
+        return reports
 
     @staticmethod
     def decode_ba_report(report):

@@ -9,9 +9,16 @@
 
 #define BA_THREADS 512
 
-__global__ void __launch_bounds__(BA_THREADS, 1) k_ba_solve(const BAParams P) {
+// one launch runs B.n independent problems, each on its own range of CTAs; a single solve is a batch of one.
+// __grid_constant__: the table is read in place, without a per-thread copy.  Each CTA copies its problem to shared
+// memory once (the body reads its per-problem pointers from there, ba_fresh); what all problems share comes from
+// problem 0 at fixed parameter offsets
+__global__ void __launch_bounds__(BA_THREADS, 1) k_ba_solve(const __grid_constant__ BABatch B) {
     extern __shared__ __align__(16) unsigned char ba_smem_raw[];
-    ba_solve_body(P, ba_smem_raw);
+    __shared__ BAParams problem;
+    if (threadIdx.x == 0) problem = B.p[ba_problem_of(B)];
+    __syncthreads();
+    ba_solve_body(problem, B.p[0], ba_smem_raw);
 }
 
 // ---- tracks -> observations --------------------------------------------------------------------------------
@@ -98,35 +105,82 @@ int ba_dev_init(mocap_ctx* ctx) {
     return MOCAP_OK;
 }
 
+// per-problem carve of the context's workspace
+struct BAProblemWS { double* X; double* Xnew; uint8_t* valid; double* part; double* fin; double* cpart; unsigned* bar; };
 struct BAWorkspace {
-    double* X; double* Xnew; uint8_t* valid; double* part; double* fin; double* cpart; unsigned* bar;
+    BAProblemWS pr[MOCAP_BA_MAX_BATCH];
     double* Rt_io; int32_t* offs; mocap_ba_report* report;
 };
 
-static int ba_workspace(mocap_ctx* ctx, int m_max, int n_sets, BAWorkspace& W, int* pstride_out) {
+#define BA_BAR_LINE 128                                           // bytes: each problem's barrier words on a line of their own
+
+// carve the workspace for K problems of m_max[k] points on g[k] CTAs (K = 0: none, the offsets of n_sets frame-sets only)
+static int ba_workspace(mocap_ctx* ctx, int K, const int* m_max, const int* g, int n_sets, BAWorkspace& W, int* pstride_out) {
     const int C = ctx->cfg.n_cam, n = 6 * (C - 1), npair = n * (n + 1) / 2;
-    const int pstride = npair + 2 * n + 8, G = ctx->ba_grid;
+    const int pstride = npair + 2 * n + 8;
     auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
-    const size_t sz[] = {al((size_t)m_max * 3 * 8), al((size_t)m_max * 3 * 8), al((size_t)m_max), al((size_t)G * pstride * 8),
-                         al((size_t)pstride * 8), al((size_t)2 * G * 4 * 8), al(256), al((size_t)C * 12 * 8),
-                         al((size_t)(n_sets > 0 ? n_sets : 1) * 4), al(sizeof(mocap_ba_report))};
-    size_t total = 0;
-    for (size_t b : sz) total += b;
+    auto problem_bytes = [&](int m, int G) {
+        return al((size_t)m * 3 * 8) + al((size_t)m * 3 * 8) + al((size_t)m) + al((size_t)G * pstride * 8) + al((size_t)pstride * 8) +
+               al((size_t)2 * G * 4 * 8);
+    };
+    const size_t bar_bytes = al((size_t)MOCAP_BA_MAX_BATCH * BA_BAR_LINE);
+    size_t total = bar_bytes + al((size_t)C * 12 * 8) + al((size_t)(n_sets > 0 ? n_sets : 1) * 4) + al(sizeof(mocap_ba_report));
+    for (int k = 0; k < K; ++k) total += problem_bytes(m_max[k], g[k]);
     if (total > ctx->ba_ws_bytes) {
         CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
         cudaFree(ctx->d_ba_ws);
         ctx->d_ba_ws = nullptr; ctx->ba_ws_bytes = 0;
         CUDA_TRY(ctx, cudaMalloc(&ctx->d_ba_ws, total));
         ctx->ba_ws_bytes = total;
-        CUDA_TRY(ctx, cudaMemsetAsync(ctx->d_ba_ws, 0, total, ctx->stream));     // the grid barrier starts at zero
+        CUDA_TRY(ctx, cudaMemsetAsync(ctx->d_ba_ws, 0, total, ctx->stream));     // the grid barriers start at zero
     }
     unsigned char* p = static_cast<unsigned char*>(ctx->d_ba_ws);
-    // the barrier words come FIRST so that they keep their place (and their generation count) when nothing grows
-    W.bar = (unsigned*)p; p += sz[6];
-    W.X = (double*)p; p += sz[0]; W.Xnew = (double*)p; p += sz[1]; W.valid = p; p += sz[2];
-    W.part = (double*)p; p += sz[3]; W.fin = (double*)p; p += sz[4]; W.cpart = (double*)p; p += sz[5];
-    W.Rt_io = (double*)p; p += sz[7]; W.offs = (int32_t*)p; p += sz[8]; W.report = (mocap_ba_report*)p;
+    // the barrier words come FIRST so that they keep their place (and their generation counts) when nothing grows
+    unsigned char* bars = p; p += bar_bytes;
+    for (int k = 0; k < K; ++k) {
+        BAProblemWS& w = W.pr[k];
+        const size_t m = (size_t)m_max[k], G = (size_t)g[k];
+        w.bar = (unsigned*)(bars + (size_t)k * BA_BAR_LINE);
+        w.X = (double*)p; p += al(m * 3 * 8); w.Xnew = (double*)p; p += al(m * 3 * 8); w.valid = p; p += al(m);
+        w.part = (double*)p; p += al(G * pstride * 8); w.fin = (double*)p; p += al((size_t)pstride * 8);
+        w.cpart = (double*)p; p += al(2 * G * 4 * 8);
+    }
+    W.Rt_io = (double*)p; p += al((size_t)C * 12 * 8); W.offs = (int32_t*)p; p += al((size_t)(n_sets > 0 ? n_sets : 1) * 4);
+    W.report = (mocap_ba_report*)p;
     *pstride_out = pstride;
+    return MOCAP_OK;
+}
+
+// one cooperative launch of k_ba_solve over the K problems (arguments checked by the caller): problem k gets
+// G / K + (k < G % K) of the context's G CTAs
+static int ba_launch(mocap_ctx* ctx, const mocap_ba_problem* pr, int K, const mocap_ba_options* opt_in) {
+    CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));
+    mocap_ba_options opt;
+    if (opt_in) opt = *opt_in; else mocap_ba_default_options(&opt);
+    const int G = ctx->ba_grid;
+    int m_max[MOCAP_BA_MAX_BATCH], g[MOCAP_BA_MAX_BATCH];
+    for (int k = 0; k < K; ++k) { m_max[k] = pr[k].n_points_max; g[k] = G / K + (k < G % K ? 1 : 0); }
+    BAWorkspace W;
+    int pstride = 0;
+    int st = ba_workspace(ctx, K, m_max, g, 0, W, &pstride);
+    if (st) return st;
+    BABatch B;
+    memset(&B, 0, sizeof(B));
+    B.n = K;
+    for (int k = 0, cta0 = 0; k < K; cta0 += g[k], ++k) {
+        BAParams& P = B.p[k];
+        const BAProblemWS& w = W.pr[k];
+        P.tb = ctx->d_tables; P.obs = pr[k].obs; P.mask = pr[k].mask; P.m_dev = pr[k].n_points; P.m_max = pr[k].n_points_max;
+        P.C = ctx->cfg.n_cam; P.R = pr[k].R; P.t = pr[k].t;
+        P.ftol = opt.ftol; P.xtol = opt.xtol; P.gtol = opt.gtol; P.max_nfev = opt.max_nfev;
+        P.jac_mode = opt.jacobian ? 1 : 0; P.prefit = opt.prefit ? 1 : 0; P.prefit_max_iter = opt.prefit_max_iter;
+        P.X = w.X; P.Xnew = w.Xnew; P.valid = w.valid; P.part = w.part; P.pstride = pstride; P.fin = w.fin; P.cpart = w.cpart;
+        P.bar = w.bar; P.report = pr[k].report;
+        P.cta0 = cta0; P.ncta = g[k];
+    }
+    void* args[] = {&B};
+    CUDA_TRY(ctx, cudaLaunchCooperativeKernel((const void*)k_ba_solve, dim3(G), dim3(ctx->ba_threads), args, ctx->ba_smem, ctx->stream));
+    ctx->launches += 1;
     return MOCAP_OK;
 }
 
@@ -152,7 +206,7 @@ int mocap_tracks_to_observations_dev(mocap_ctx* ctx, const int32_t* track_xy, co
     BAWorkspace W;
     int pstride = 0;
     if (ctx->ba_grid < 1) return mocap_fail(ctx, MOCAP_EINVAL, "bundle adjustment needs at least two cameras");
-    int st = ba_workspace(ctx, 1, n_frame_sets, W, &pstride);
+    int st = ba_workspace(ctx, 0, nullptr, nullptr, n_frame_sets, W, &pstride);
     if (st) return st;
     const int RM = ctx->cfg.max_roots, C = ctx->cfg.n_cam;
     k_track_offsets<<<1, 1024, 0, ctx->stream>>>(n_obj, err, n_frame_sets, RM, max_err, capacity, W.offs, n_points);
@@ -174,25 +228,26 @@ int mocap_bundle_adjust_dev(mocap_ctx* ctx, const double* obs, const uint8_t* ma
     if (!ctx->cameras_set) return mocap_fail(ctx, MOCAP_ESTATE, "mocap_set_cameras has not been called (intrinsics are needed)");
     if (ctx->cfg.n_cam < 2) return mocap_fail(ctx, MOCAP_EINVAL, "bundle adjustment needs at least two cameras");
     if (ctx->ba_grid < 1) return mocap_fail(ctx, MOCAP_EINVAL, "k_ba_solve needs %zu bytes of shared memory per CTA for %d cameras", ctx->ba_smem, ctx->cfg.n_cam);
-    CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));
-    mocap_ba_options opt;
-    if (opt_in) opt = *opt_in; else mocap_ba_default_options(&opt);
-    BAWorkspace W;
-    BAParams P;
-    memset(&P, 0, sizeof(P));
-    // keep the offsets buffer of a preceding mocap_tracks_to_observations_dev call in place: size for the larger of the two
-    int st = ba_workspace(ctx, n_points_max, 0, W, &P.pstride);
-    if (st) return st;
-    P.tb = ctx->d_tables; P.obs = obs; P.mask = mask; P.m_dev = n_points; P.m_max = n_points_max; P.C = ctx->cfg.n_cam;
-    P.R = R; P.t = t;
-    P.ftol = opt.ftol; P.xtol = opt.xtol; P.gtol = opt.gtol; P.max_nfev = opt.max_nfev;
-    P.jac_mode = opt.jacobian ? 1 : 0; P.prefit = opt.prefit ? 1 : 0; P.prefit_max_iter = opt.prefit_max_iter;
-    P.X = W.X; P.Xnew = W.Xnew; P.valid = W.valid; P.part = W.part; P.fin = W.fin; P.cpart = W.cpart; P.bar = W.bar;
-    P.report = report;
-    void* args[] = {&P};
-    CUDA_TRY(ctx, cudaLaunchCooperativeKernel((const void*)k_ba_solve, dim3(ctx->ba_grid), dim3(ctx->ba_threads), args, ctx->ba_smem, ctx->stream));
-    ctx->launches += 1;
-    return MOCAP_OK;
+    // a batch of one on all the context's CTAs
+    const mocap_ba_problem pr = {obs, mask, n_points_max, n_points, R, t, report};
+    return ba_launch(ctx, &pr, 1, opt_in);
+}
+
+int mocap_bundle_adjust_batch_dev(mocap_ctx* ctx, const mocap_ba_problem* problems, int n_problems, const mocap_ba_options* opt) {
+    if (!ctx) return MOCAP_EINVAL;
+    if (!problems) return mocap_fail(ctx, MOCAP_EINVAL, "mocap_bundle_adjust_batch_dev: problems is NULL");
+    if (!ctx->cameras_set) return mocap_fail(ctx, MOCAP_ESTATE, "mocap_set_cameras has not been called (intrinsics are needed)");
+    if (ctx->cfg.n_cam < 2) return mocap_fail(ctx, MOCAP_EINVAL, "bundle adjustment needs at least two cameras");
+    if (ctx->ba_grid < 1) return mocap_fail(ctx, MOCAP_EINVAL, "k_ba_solve needs %zu bytes of shared memory per CTA for %d cameras", ctx->ba_smem, ctx->cfg.n_cam);
+    if (n_problems < 1 || n_problems > MOCAP_BA_MAX_BATCH || n_problems > ctx->ba_grid)
+        return mocap_fail(ctx, MOCAP_EINVAL, "mocap_bundle_adjust_batch_dev: %d problems, 1 .. %d possible (MOCAP_BA_MAX_BATCH, and at most the %d CTAs of the context)",
+                          n_problems, MOCAP_BA_MAX_BATCH < ctx->ba_grid ? MOCAP_BA_MAX_BATCH : ctx->ba_grid, ctx->ba_grid);
+    for (int k = 0; k < n_problems; ++k) {
+        const mocap_ba_problem& p = problems[k];
+        if (!p.obs || !p.mask || !p.R || !p.t || p.n_points_max <= 0)
+            return mocap_fail(ctx, MOCAP_EINVAL, "mocap_bundle_adjust_batch_dev: bad argument in problem %d", k);
+    }
+    return ba_launch(ctx, problems, n_problems, opt);
 }
 
 }  // extern "C"

@@ -8,7 +8,7 @@
 // accept / reject logic all run inside k_ba_solve.
 //
 // Organisation
-//   * points are cut into tiles; tile T belongs to CTA T mod gridDim.x for the whole solve, so a point's 3D
+//   * points are cut into tiles; tile T belongs to CTA T mod ncta for the whole solve, so a point's 3D
 //     estimate never leaves its CTA;
 //   * a CTA turns a tile into rows of a small dense system in SHARED memory (prefit: the three rows
 //     Z = W L^-T of every point's eliminated 3x3 block plus its per-camera 2x6 Jacobians; polish: the robust-scaled
@@ -21,6 +21,10 @@
 //     A + alpha I instead of scipy's SVD -- the same phi(alpha), phi'(alpha)), so that the step, the trial poses and
 //     every accept / reject decision are bit-identical on all CTAs and need no broadcast;
 //   * trial points cost one residual pass and one grid barrier.
+// "The grid" above is the problem's SUB-grid: one launch can run several independent problems (BABatch), each on
+// its own contiguous range of CTAs with its own barrier words and workspace.  The body never uses blockIdx / gridDim
+// directly but the CTA's index and count within its problem (BACtrl::cta / ncta), so that a problem gives the same
+// bits on a sub-grid of g CTAs as alone on a grid of g CTAs.
 // The code is written against threadIdx / blockIdx / blockDim / gridDim and ba_grid_sync() only, so that
 // tests/hostcheck runs it unchanged on the host (several CTAs of real threads) against the host-stepped model.
 #pragma once
@@ -59,16 +63,24 @@ struct BAParams {
     double* cpart;                 // [2][grid][4] trial-point partials (cost, non-finite, count)
     unsigned* bar;                 // [2] grid barrier: arrivals, generation
     mocap_ba_report* report;       // device, may be nullptr
+    int cta0, ncta;                // this problem's CTAs of the launch: [cta0, cta0 + ncta); ncta == 0: the whole grid
+};
+
+// the problems of one launch: problem k owns CTAs [p[k].cta0, p[k].cta0 + p[k].ncta), in increasing k
+struct BABatch {
+    int n;
+    BAParams p[MOCAP_BA_MAX_BATCH];
 };
 
 #if defined(__CUDA_ARCH__)
 #define BA_DEV __device__ __forceinline__
-__device__ __forceinline__ void ba_grid_sync(unsigned* bar) {
+// barrier of the n CTAs that share the words bar (arrivals, generation)
+__device__ __forceinline__ void ba_grid_sync(unsigned* bar, unsigned n) {
     __syncthreads();
     if (threadIdx.x == 0) {
         __threadfence();
         const unsigned gen = *reinterpret_cast<volatile unsigned*>(bar + 1);
-        if (atomicAdd(bar, 1u) == gridDim.x - 1) {
+        if (atomicAdd(bar, 1u) == n - 1) {
             bar[0] = 0;
             __threadfence();
             atomicAdd(bar + 1, 1u);
@@ -81,11 +93,33 @@ __device__ __forceinline__ void ba_grid_sync(unsigned* bar) {
 }
 #elif defined(__CUDACC__)
 #define BA_DEV __device__ __forceinline__
-__device__ __forceinline__ void ba_grid_sync(unsigned*) {}
+__device__ __forceinline__ void ba_grid_sync(unsigned*, unsigned) {}
 #else
 #define BA_DEV static inline
-static inline void ba_grid_sync(unsigned*) { simt_grid_sync(); }
+// host emulation (tests/hostcheck/simt_emu.h): the device's counter-and-generation scheme, waiting with a yield, so
+// that sub-grids which iterate different numbers of times do not wait for each other
+static inline void ba_grid_sync(unsigned* bar, unsigned n) {
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        const unsigned gen = __atomic_load_n(bar + 1, __ATOMIC_SEQ_CST);
+        if (__atomic_fetch_add(bar, 1u, __ATOMIC_SEQ_CST) == n - 1) {
+            __atomic_store_n(bar, 0u, __ATOMIC_SEQ_CST);
+            __atomic_fetch_add(bar + 1, 1u, __ATOMIC_SEQ_CST);
+        } else {
+            while (__atomic_load_n(bar + 1, __ATOMIC_SEQ_CST) == gen) std::this_thread::yield();
+        }
+    }
+    __syncthreads();
+}
 #endif
+
+// index of this CTA's problem in the launch
+BA_DEV int ba_problem_of(const BABatch& B) {
+    int k = 0;
+#pragma unroll
+    for (int q = 1; q < MOCAP_BA_MAX_BATCH; ++q) k += (q < B.n && (int)blockIdx.x >= B.p[q].cta0) ? 1 : 0;
+    return k;
+}
 
 // ---- parameterisation (scipy.spatial.transform.Rotation as the reference uses it, helpers.py:247-262, 278-285;
 //      same arithmetic as trf_core.h) --------------------------------------------------------------------------
@@ -318,6 +352,7 @@ struct BACtrl {
     double pf_cost0, pf_cost1;
     double tr_alpha, tr_lower, tr_upper, tr_conv, a_diag, hh_beta, hh_alpha, hh_K;
     int m, ntiles, n_valid, nfev, njev, iteration, termination, finite, flag, go, pf_it, accepted, tr_its, tr_calls;
+    int cta, ncta;                     // this CTA's index in its problem's sub-grid, and the sub-grid's size
 };
 
 struct BAShared {
@@ -400,14 +435,19 @@ BA_DEV BAShared ba_carve(unsigned char* raw, int C, int nt) {
     return s;
 }
 
-// this CTA's points: local index i -> global point (tile T = blockIdx.x + (i / BA_TILE) * gridDim.x)
-BA_DEV int ba_local_tiles(int ntiles) {
-    const int b = blockIdx.x, G = gridDim.x;
+// a value of this CTA's problem (or of BACtrl) read afresh at every use.  k_ba_solve stages the CTA's problem in shared
+// memory; a pointer that is reloaded (one shared load) where it is used holds no register across the hot loops, which
+// keeps the kernel's spills at or below those of the kernel that read a single problem from its parameter
+template <typename T> BA_DEV T ba_fresh(const T& v) { return *const_cast<const volatile T*>(&v); }
+
+// this CTA's points: local index i -> global point (tile T = cta + (i / BA_TILE) * ncta)
+BA_DEV int ba_local_tiles(const BACtrl* ctl) {
+    const int b = ba_fresh(ctl->cta), G = ba_fresh(ctl->ncta), ntiles = ctl->ntiles;
     return ntiles > b ? (ntiles - b + G - 1) / G : 0;
 }
-BA_DEV int ba_point_of(int local_index) {
+BA_DEV int ba_point_of(const BACtrl* ctl, int local_index) {
     const int lt = local_index / BA_TILE;
-    return ((int)blockIdx.x + lt * (int)gridDim.x) * BA_TILE + (local_index - lt * BA_TILE);
+    return (ba_fresh(ctl->cta) + lt * ba_fresh(ctl->ncta)) * BA_TILE + (local_index - lt * BA_TILE);
 }
 
 // CTA-wide sum of per-thread values, fixed order (thread 0 adds the warps' partial sums held in `scratch`)
@@ -429,23 +469,26 @@ BA_DEV double ba_block_sum(double v, double* scratch) {
 // ---- passes over this CTA's points ---------------------------------------------------------------------------
 // reference objective at the poses Rt: 0.5 * sum log1p(f^2) over the CTA's valid points (+ non-finite flag);
 // optionally marks valid points and stores the DLT points (start of the prefit)
-BA_DEV void ba_cost_pass(const BAParams& P, const BAShared& S, const double* Rt, bool first, double* scratch, double out[3]) {
-    const int tid = threadIdx.x, nt = blockDim.x, C = P.C;
-    const int m = S.ctl->m, lt = ba_local_tiles(S.ctl->ntiles);
+BA_DEV void ba_cost_pass(const BAParams& P, const BAParams& Q, const BAShared& S, const double* Rt, bool first, double* scratch, double out[3]) {
+    const int tid = threadIdx.x, nt = blockDim.x, C = Q.C;
+    const int lt = ba_local_tiles(S.ctl);
     double c = 0.0, bad = 0.0, cnt = 0.0;
+    const uint8_t* mask = ba_fresh(P.mask);
+    const double* obs = ba_fresh(P.obs);
+    uint8_t* valid = ba_fresh(P.valid);
     for (int i = tid; i < lt * BA_TILE; i += nt) {
-        const int p = ba_point_of(i);
-        if (p >= m) continue;
-        const uint8_t* mk = P.mask + (size_t)p * C;
+        const int p = ba_point_of(S.ctl, i);
+        if (p >= ba_fresh(S.ctl->m)) continue;
+        const uint8_t* mk = mask + (size_t)p * C;
         if (first) {
             int nv = 0;
             for (int k = 0; k < C; ++k) nv += mk[k] ? 1 : 0;
-            P.valid[p] = nv > 1 ? 1 : 0;                       // helpers.py:207-208,222-223: <= 1 view is skipped
+            valid[p] = nv > 1 ? 1 : 0;             // helpers.py:207-208,222-223: <= 1 view is skipped
         }
-        if (!P.valid[p]) continue;
+        if (!valid[p]) continue;
         double X[3];
-        const double r = ba_residual(P.tb, Rt, -1, nullptr, P.obs + (size_t)p * C * 2, mk, C, X);
-        if (first) { P.X[3 * p] = X[0]; P.X[3 * p + 1] = X[1]; P.X[3 * p + 2] = X[2]; }
+        const double r = ba_residual(Q.tb, Rt, -1, nullptr, obs + (size_t)p * C * 2, mk, C, X);
+        if (first) { ba_fresh(P.X)[3 * p] = X[0]; ba_fresh(P.X)[3 * p + 1] = X[1]; ba_fresh(P.X)[3 * p + 2] = X[2]; }
         const float fv = (float)r;                             // helpers.py:273
         if (!isfinite(fv)) bad = 1.0;
         c += (double)log1pf(fv * fv);
@@ -458,10 +501,10 @@ BA_DEV void ba_cost_pass(const BAParams& P, const BAShared& S, const double* Rt,
 
 // publish 3 numbers of this CTA, grid barrier, read the grid totals (every CTA sums in CTA order)
 BA_DEV void ba_grid_sum3(const BAParams& P, const BAShared& S, int slot, const double v[3], double tot[3]) {
-    const int G = gridDim.x;
-    double* cp = P.cpart + (size_t)slot * G * 4;
-    if (threadIdx.x == 0) { cp[4 * blockIdx.x] = v[0]; cp[4 * blockIdx.x + 1] = v[1]; cp[4 * blockIdx.x + 2] = v[2]; }
-    ba_grid_sync(P.bar);
+    const int G = S.ctl->ncta, b = S.ctl->cta;
+    double* cp = ba_fresh(P.cpart) + (size_t)slot * G * 4;
+    if (threadIdx.x == 0) { cp[4 * b] = v[0]; cp[4 * b + 1] = v[1]; cp[4 * b + 2] = v[2]; }
+    ba_grid_sync(ba_fresh(P.bar), G);
     if (threadIdx.x < 3) {                                         // one thread per component, in CTA order; the CTA shares the result
         double a = 0.0;
         for (int g = 0; g < G; ++g) a += __ldcg(cp + 4 * g + threadIdx.x);
@@ -473,10 +516,10 @@ BA_DEV void ba_grid_sum3(const BAParams& P, const BAShared& S, int slot, const d
 }
 
 // write this CTA's partial system, grid barrier, add a slice of the entries over all CTAs, grid barrier
-BA_DEV void ba_reduce_system(const BAParams& P, const BAShared& S, int n_entries) {
-    const int tid = threadIdx.x, nt = blockDim.x, G = gridDim.x, b = blockIdx.x;
-    for (int e = tid; e < n_entries; e += nt) P.part[(size_t)b * P.pstride + e] = S.acc[e];
-    ba_grid_sync(P.bar);
+BA_DEV void ba_reduce_system(const BAParams& P, const BAParams& Q, const BAShared& S, int n_entries) {
+    const int tid = threadIdx.x, nt = blockDim.x, G = S.ctl->ncta, b = S.ctl->cta;
+    for (int e = tid; e < n_entries; e += nt) ba_fresh(P.part)[(size_t)b * Q.pstride + e] = S.acc[e];
+    ba_grid_sync(ba_fresh(P.bar), G);
     // every CTA adds its slice of the entries over all CTAs: W threads per entry fetch the partials side by side
     // (the few loads of one thread are independent), then one thread adds the W sub-sums in a fixed order
     const int per = (n_entries + G - 1) / G;
@@ -486,26 +529,26 @@ BA_DEV void ba_reduce_system(const BAParams& P, const BAShared& S, int n_entries
         const int e = base + tid / Wd, j = tid % Wd;
         double s = 0.0;
         if (e < e1 && tid / Wd < nt / Wd)
-            for (int g = j; g < G; g += Wd) s += P.part[(size_t)g * P.pstride + e];
+            for (int g = j; g < G; g += Wd) s += ba_fresh(P.part)[(size_t)g * Q.pstride + e];
         __syncthreads();
         S.scratch[tid] = s;
         __syncthreads();
         if (j == 0 && e < e1 && tid / Wd < nt / Wd) {
             double t = 0.0;
             for (int q = 0; q < Wd; ++q) t += S.scratch[tid + q];
-            P.fin[e] = t;
+            ba_fresh(P.fin)[e] = t;
         }
     }
-    ba_grid_sync(P.bar);
+    ba_grid_sync(ba_fresh(P.bar), G);
 }
 
 // ---- prefit: Levenberg-Marquardt over poses and points --------------------------------------------------------
 // accumulate the reduced camera system of this CTA's points at (S.Rt, P.X) with damping lambda into S.acc:
 // [0, npair) S (upper pairs), [npair, npair+n) r, [npair+n, npair+2n) D, [npair+2n] cost
-BA_DEV void ba_prefit_accumulate(const BAParams& P, const BAShared& S, double lambda) {
-    const int tid = threadIdx.x, nt = blockDim.x, C = P.C, n = 6 * (C - 1), npair = n * (n + 1) / 2;
+BA_DEV void ba_prefit_accumulate(const BAParams& P, const BAParams& Q, const BAShared& S, double lambda) {
+    const int tid = threadIdx.x, nt = blockDim.x, C = Q.C, n = 6 * (C - 1), npair = n * (n + 1) / 2;
     const int Pp = ba_prefit_points(C, nt);
-    const int m = S.ctl->m, lt = ba_local_tiles(S.ctl->ntiles);
+    const int lt = ba_local_tiles(S.ctl);
     // tile buffers
     double* Z = reinterpret_cast<double*>(S.uni);                 // [3*Pp][n]
     double* Jc = Z + (size_t)3 * Pp * n;                           // [Pp][C][12]
@@ -519,20 +562,20 @@ BA_DEV void ba_prefit_accumulate(const BAParams& P, const BAShared& S, double la
     for (int e = tid; e < npair + 2 * n + 1; e += nt) S.acc[e] = 0.0;
     const int sub = BA_TILE / Pp;                                  // a BA_TILE tile is walked in `sub` pieces of Pp points
     for (int l = 0; l < lt * sub; ++l) {
-        const int base = ba_point_of((l / sub) * BA_TILE) + (l % sub) * Pp;
+        const int base = ba_point_of(S.ctl, (l / sub) * BA_TILE) + (l % sub) * Pp;
         __syncthreads();
         for (int e = tid; e < 3 * Pp * n; e += nt) Z[e] = 0.0;
         // (point, view): Jacobians
         for (int it = tid; it < Pp * C; it += nt) {
             const int c = it / Pp, pt = it - c * Pp, p = base + pt;
             bool pr = false;
-            if (p < m && P.valid[p] && P.mask[(size_t)p * C + c]) {
+            if (p < ba_fresh(S.ctl->m) && ba_fresh(P.valid)[p] && ba_fresh(P.mask)[(size_t)p * C + c]) {
                 int k = 0;
-                for (int cc = 0; cc < c; ++cc) k += P.mask[(size_t)p * C + cc] ? 1 : 0;
-                const double Xp[3] = {P.X[3 * p], P.X[3 * p + 1], P.X[3 * p + 2]};
+                for (int cc = 0; cc < c; ++cc) k += ba_fresh(P.mask)[(size_t)p * C + cc] ? 1 : 0;
+                const double Xp[3] = {ba_fresh(P.X)[3 * p], ba_fresh(P.X)[3 * p + 1], ba_fresh(P.X)[3 * p + 2]};
                 BAViewJac J;
-                ba_view_jacobian(S.Rt + 12 * c, P.tb->fx[k], P.tb->fy[k], P.tb->cx[k], P.tb->cy[k], Xp,
-                                 P.obs[((size_t)p * C + c) * 2], P.obs[((size_t)p * C + c) * 2 + 1], J);
+                ba_view_jacobian(S.Rt + 12 * c, Q.tb->fx[k], Q.tb->fy[k], Q.tb->cx[k], Q.tb->cy[k], Xp,
+                                 ba_fresh(P.obs)[((size_t)p * C + c) * 2], ba_fresh(P.obs)[((size_t)p * C + c) * 2 + 1], J);
                 double* jc = Jc + ((size_t)pt * C + c) * 12;
                 double* jp = Jp + ((size_t)pt * C + c) * 6;
                 for (int a = 0; a < 6; ++a) { jc[a] = J.Jc[0][a]; jc[6 + a] = J.Jc[1][a]; }
@@ -653,7 +696,7 @@ BA_DEV void ba_prefit_accumulate(const BAParams& P, const BAShared& S, double la
         }
         if (tid == 0) {
             double cst = 0.0;
-            for (int pt = 0; pt < Pp; ++pt) if (base + pt < m && P.valid[base + pt]) cst += pc[pt];
+            for (int pt = 0; pt < Pp; ++pt) if (base + pt < ba_fresh(S.ctl->m) && ba_fresh(P.valid)[base + pt]) cst += pc[pt];
             S.acc[npair + 2 * n] += cst;
         }
     }
@@ -662,21 +705,23 @@ BA_DEV void ba_prefit_accumulate(const BAParams& P, const BAShared& S, double la
 
 // back-substitution of this CTA's points for the camera step dc (S.p) at (S.Rt, P.X) -> P.Xnew, and
 // 0.5 * squared pixel residuals at (S.Rt_new, P.Xnew)
-BA_DEV double ba_prefit_backsub(const BAParams& P, const BAShared& S, double lambda, double* scratch) {
-    const int tid = threadIdx.x, nt = blockDim.x, C = P.C;
-    const int m = S.ctl->m, lt = ba_local_tiles(S.ctl->ntiles);
+BA_DEV double ba_prefit_backsub(const BAParams& P, const BAParams& Q, const BAShared& S, double lambda, double* scratch) {
+    const int tid = threadIdx.x, nt = blockDim.x, C = Q.C;
+    const int lt = ba_local_tiles(S.ctl);
     double cst = 0.0;
+    const uint8_t* const mask = ba_fresh(P.mask);
+    const double* const obs = ba_fresh(P.obs);
     for (int i = tid; i < lt * BA_TILE; i += nt) {
-        const int p = ba_point_of(i);
-        if (p >= m || !P.valid[p]) continue;
-        const double Xp[3] = {P.X[3 * p], P.X[3 * p + 1], P.X[3 * p + 2]};
+        const int p = ba_point_of(S.ctl, i);
+        if (p >= ba_fresh(S.ctl->m) || !ba_fresh(P.valid)[p]) continue;
+        const double Xp[3] = {ba_fresh(P.X)[3 * p], ba_fresh(P.X)[3 * p + 1], ba_fresh(P.X)[3 * p + 2]};
         double H[6] = {0, 0, 0, 0, 0, 0}, rhs[3] = {0, 0, 0};
         int k = 0;
         for (int c = 0; c < C; ++c) {
-            if (!P.mask[(size_t)p * C + c]) continue;
+            if (!mask[(size_t)p * C + c]) continue;
             BAViewJac J;
-            ba_view_jacobian(S.Rt + 12 * c, P.tb->fx[k], P.tb->fy[k], P.tb->cx[k], P.tb->cy[k], Xp,
-                             P.obs[((size_t)p * C + c) * 2], P.obs[((size_t)p * C + c) * 2 + 1], J);
+            ba_view_jacobian(S.Rt + 12 * c, Q.tb->fx[k], Q.tb->fy[k], Q.tb->cx[k], Q.tb->cy[k], Xp,
+                             obs[((size_t)p * C + c) * 2], obs[((size_t)p * C + c) * 2 + 1], J);
             ++k;
             H[0] += J.Jp[0][0] * J.Jp[0][0] + J.Jp[1][0] * J.Jp[1][0]; H[1] += J.Jp[0][0] * J.Jp[0][1] + J.Jp[1][0] * J.Jp[1][1];
             H[2] += J.Jp[0][0] * J.Jp[0][2] + J.Jp[1][0] * J.Jp[1][2]; H[3] += J.Jp[0][1] * J.Jp[0][1] + J.Jp[1][1] * J.Jp[1][1];
@@ -704,16 +749,16 @@ BA_DEV double ba_prefit_backsub(const BAParams& P, const BAShared& S, double lam
             }
         }
         const double Xn[3] = {Xp[0] - dp[0], Xp[1] - dp[1], Xp[2] - dp[2]};
-        P.Xnew[3 * p] = Xn[0]; P.Xnew[3 * p + 1] = Xn[1]; P.Xnew[3 * p + 2] = Xn[2];
+        ba_fresh(P.Xnew)[3 * p] = Xn[0]; ba_fresh(P.Xnew)[3 * p + 1] = Xn[1]; ba_fresh(P.Xnew)[3 * p + 2] = Xn[2];
         k = 0;
         for (int c = 0; c < C; ++c)
-            if (P.mask[(size_t)p * C + c]) {
+            if (mask[(size_t)p * C + c]) {
                 const double* Rt = S.Rt_new + 12 * c;
                 const double x = Rt[0] * Xn[0] + Rt[1] * Xn[1] + Rt[2] * Xn[2] + Rt[3];
                 const double y = Rt[4] * Xn[0] + Rt[5] * Xn[1] + Rt[6] * Xn[2] + Rt[7];
                 const double z = Rt[8] * Xn[0] + Rt[9] * Xn[1] + Rt[10] * Xn[2] + Rt[11];
-                const double eu = P.tb->fx[k] * x / z + P.tb->cx[k] - P.obs[((size_t)p * C + c) * 2];
-                const double ev = P.tb->fy[k] * y / z + P.tb->cy[k] - P.obs[((size_t)p * C + c) * 2 + 1];
+                const double eu = Q.tb->fx[k] * x / z + Q.tb->cx[k] - obs[((size_t)p * C + c) * 2];
+                const double ev = Q.tb->fy[k] * y / z + Q.tb->cy[k] - obs[((size_t)p * C + c) * 2 + 1];
                 cst += eu * eu + ev * ev;
                 ++k;
             }
@@ -723,8 +768,8 @@ BA_DEV double ba_prefit_backsub(const BAParams& P, const BAShared& S, double lam
 
 // ---- polish: scipy's trust-region iteration on the reference objective ------------------------------------------
 // finite-difference columns at S.x (scipy _compute_absolute_step / 2-point): colRt, colcam, dx
-BA_DEV void ba_make_columns(const BAParams& P, const BAShared& S) {
-    const int tid = threadIdx.x, nt = blockDim.x, C = P.C, n = 6 * (C - 1);
+BA_DEV void ba_make_columns(const BAParams& P, const BAParams& Q, const BAShared& S) {
+    const int tid = threadIdx.x, nt = blockDim.x, C = Q.C, n = 6 * (C - 1);
     for (int j = tid; j < n; j += nt) {
         const int cam = 1 + j / 6, idx = 1 + 7 * (cam - 1) + 1 + j % 6;
         double xq[7];
@@ -745,26 +790,30 @@ BA_DEV void ba_make_columns(const BAParams& P, const BAShared& S) {
 
 // robust-scaled normal equations of this CTA's points at S.x (S.Rt holds its poses) into S.acc:
 // [0, npair) J^T J (upper pairs), [npair, npair+n) J^T f, [npair+n] cost, [npair+n+1] non-finite
-BA_DEV void ba_polish_accumulate(const BAParams& P, const BAShared& S) {
-    const int tid = threadIdx.x, nt = blockDim.x, C = P.C, n = 6 * (C - 1), npair = n * (n + 1) / 2, ncol = n + 1;
-    const int m = S.ctl->m, lt = ba_local_tiles(S.ctl->ntiles);
+BA_DEV void ba_polish_accumulate(const BAParams& P, const BAParams& Q, const BAShared& S) {
+    const int tid = threadIdx.x, nt = blockDim.x, C = Q.C, n = 6 * (C - 1), npair = n * (n + 1) / 2, ncol = n + 1;
+    const int lt = ba_local_tiles(S.ctl);
     double* F = reinterpret_cast<double*>(S.uni);                  // [BA_TILE][ncol] residuals, then the scaled Jacobian rows
     double* fs = F + (size_t)BA_TILE * ncol;                        // [BA_TILE] scaled residual
     double* ct = fs + BA_TILE;                                      // [BA_TILE] log1p(f^2)
     for (int e = tid; e < npair + n + 2; e += nt) S.acc[e] = 0.0;
     for (int l = 0; l < lt; ++l) {
-        const int base = ba_point_of(l * BA_TILE);
+        const int base = ba_point_of(S.ctl, l * BA_TILE);
+        const uint8_t* const mask = ba_fresh(P.mask);
+        const double* const obs = ba_fresh(P.obs);
+        const uint8_t* const valid = ba_fresh(P.valid);
+        const int m = ba_fresh(S.ctl->m);
         __syncthreads();
         // (column, point): one warp = one column of the tile
         for (int it = tid; it < BA_TILE * ncol; it += nt) {
             const int col = it / BA_TILE, pt = it - col * BA_TILE, p = base + pt;
             double r = 0.0;
-            if (p < m && P.valid[p]) {
-                const uint8_t* mk = P.mask + (size_t)p * C;
+            if (p < m && valid[p]) {
+                const uint8_t* mk = mask + (size_t)p * C;
                 const int cam = col == 0 ? -1 : S.colcam[col - 1];
                 if (cam < 0 || mk[cam]) {                          // a column that touches no view of the point: difference 0
                     double X[3];
-                    r = ba_residual(P.tb, S.Rt, cam, cam < 0 ? nullptr : S.colRt + 12 * (col - 1), P.obs + (size_t)p * C * 2, mk, C, X);
+                    r = ba_residual(Q.tb, S.Rt, cam, cam < 0 ? nullptr : S.colRt + 12 * (col - 1), obs + (size_t)p * C * 2, mk, C, X);
                 }
             }
             F[(size_t)pt * ncol + col] = r;
@@ -774,12 +823,12 @@ BA_DEV void ba_polish_accumulate(const BAParams& P, const BAShared& S) {
         for (int pt = tid; pt < BA_TILE; pt += nt) {
             const int p = base + pt;
             double* row = F + (size_t)pt * ncol;
-            if (!(p < m && P.valid[p])) {
+            if (!(p < m && valid[p])) {
                 fs[pt] = 0.0; ct[pt] = 0.0;
                 for (int j = 0; j < n; ++j) row[j] = 0.0;
                 continue;
             }
-            const uint8_t* mk = P.mask + (size_t)p * C;
+            const uint8_t* mk = mask + (size_t)p * C;
             const double f0d = row[0];
             const float fv = (float)f0d;
             if (!isfinite(fv)) S.acc[npair + n + 1] = 1.0;          // any writer stores the same value
@@ -793,7 +842,7 @@ BA_DEV void ba_polish_accumulate(const BAParams& P, const BAShared& S) {
             for (int j = 0; j < n; ++j) {                          // in place: entry j is written after entry j + 1 was read
                 double Jv = 0.0;
                 if (mk[S.colcam[j]]) {
-                    if (P.jac_mode == 0) Jv = (double)((float)row[j + 1] - fv) / S.dx[j];
+                    if (Q.jac_mode == 0) Jv = (double)((float)row[j + 1] - fv) / S.dx[j];
                     else Jv = (row[j + 1] - f0d) / S.dx[j];
                 }
                 row[j] = Jv * js;
@@ -833,10 +882,10 @@ BA_DEV void ba_load_system(const BAParams& P, const BAShared& S, int n) {
     __syncthreads();
     for (int k = tid; k < npair; k += nt) {
         const int i = S.pi[k], j = S.pj[k];
-        const double v = P.fin[k];
+        const double v = ba_fresh(P.fin)[k];
         S.A[(size_t)i * n + j] = v; S.A[(size_t)j * n + i] = v;
     }
-    for (int i = tid; i < n; i += nt) S.g[i] = P.fin[npair + i];
+    for (int i = tid; i < n; i += nt) S.g[i] = ba_fresh(P.fin)[npair + i];
     __syncthreads();
     if (tid == 0) {
         double d = 0.0;
@@ -1056,9 +1105,12 @@ BA_DEV void ba_solve_tr(const BAShared& S, int n) {
     __syncthreads();
 }
 
-// the whole solve; every CTA runs the same control flow on the same numbers
-BA_DEV void ba_solve_body(const BAParams& P, unsigned char* smem) {
-    const int tid = threadIdx.x, nt = blockDim.x, C = P.C;
+// the whole solve; every CTA runs the same control flow on the same numbers.
+// P: this CTA's problem.  Q: any problem of the launch, read ONLY for what all of them share (cameras, options,
+// pstride): in a batched launch Q is problem 0, whose fields sit at fixed offsets of the kernel parameter, so that
+// the hot loops read them as constants instead of through the per-CTA problem index
+BA_DEV void ba_solve_body(const BAParams& P, const BAParams& Q, unsigned char* smem) {
+    const int tid = threadIdx.x, nt = blockDim.x, C = Q.C;
     const int n = 6 * (C - 1), nf = 1 + 7 * (C - 1), npair = n * (n + 1) / 2;
     const BAShared S = ba_carve(smem, C, nt);
     BACtrl* ctl = S.ctl;
@@ -1070,7 +1122,8 @@ BA_DEV void ba_solve_body(const BAParams& P, unsigned char* smem) {
         if (m > P.m_max) m = P.m_max;
         if (m < 0) m = 0;
         ctl->m = m; ctl->ntiles = (m + BA_TILE - 1) / BA_TILE;
-        S.x[0] = P.tb->Kmat[0][0];
+        ctl->cta = (int)blockIdx.x - P.cta0; ctl->ncta = P.ncta > 0 ? P.ncta : (int)gridDim.x;
+        S.x[0] = Q.tb->Kmat[0][0];
     }
     for (int k = tid; k < npair; k += nt) {                        // pair table: k -> (i, j), i <= j, row by row
         int i = 0, rem = k;
@@ -1079,7 +1132,7 @@ BA_DEV void ba_solve_body(const BAParams& P, unsigned char* smem) {
     }
     for (int c = 1 + tid; c < C; c += nt) {                        // helpers.py:278-285
         double* q = S.x + 1 + 7 * (c - 1);
-        q[0] = P.tb->Kmat[c - 1][0];
+        q[0] = Q.tb->Kmat[c - 1][0];
         ba_matrix_to_rotvec(P.R + 9 * c, q + 1);
         q[4] = P.t[3 * c]; q[5] = P.t[3 * c + 1]; q[6] = P.t[3 * c + 2];
     }
@@ -1090,7 +1143,7 @@ BA_DEV void ba_solve_body(const BAParams& P, unsigned char* smem) {
     if (tid == 0) { for (int k = 0; k < 8; ++k) ctl->prof[k] = 0; ctl->t_last = ba_clock(); }
     // reference objective and DLT points at the start
     double v3[3], tot[3];
-    ba_cost_pass(P, S, S.Rt, true, scratch, v3);
+    ba_cost_pass(P, Q, S, S.Rt, true, scratch, v3);
     ba_grid_sum3(P, S, slot, v3, tot); slot ^= 1;
     if (tid == 0) {
         ctl->cost_initial = tot[0]; ctl->cost = tot[0]; ctl->finite = tot[1] == 0.0; ctl->n_valid = (int)tot[2];
@@ -1099,7 +1152,7 @@ BA_DEV void ba_solve_body(const BAParams& P, unsigned char* smem) {
     }
     __syncthreads();
     if (ctl->n_valid == 0) {
-        if (blockIdx.x == 0 && tid == 0 && P.report) {
+        if (ctl->cta == 0 && tid == 0 && P.report) {
             mocap_ba_report r;
             r.cost_initial = 0; r.cost_final = 0; r.optimality = 0; r.n_iterations = 0; r.n_fev = 0; r.status = -3; r.n_residuals = 0;
             r.prefit_cost_initial = 0; r.prefit_cost_final = 0; r.prefit_iterations = 0; r.n_launches = 1;
@@ -1111,8 +1164,8 @@ BA_DEV void ba_solve_body(const BAParams& P, unsigned char* smem) {
     }
 
     // ---- prefit ------------------------------------------------------------------------------------------------
-    if (P.prefit) {
-        const int max_iter = P.prefit_max_iter > 0 ? P.prefit_max_iter : 50;
+    if (Q.prefit) {
+        const int max_iter = Q.prefit_max_iter > 0 ? Q.prefit_max_iter : 50;
         if (tid == 0) { ctl->lambda = 1e-3; ctl->go = 1; ctl->pcost = -1.0; }
         __syncthreads();
         int it = 0;
@@ -1120,19 +1173,19 @@ BA_DEV void ba_solve_body(const BAParams& P, unsigned char* smem) {
             const double lambda = ctl->lambda;
             __syncthreads();                                       // everybody has read go / lambda
             BA_TICK(BA_PH_SETUP);
-            ba_prefit_accumulate(P, S, lambda);
-            ba_reduce_system(P, S, npair + 2 * n + 1);
+            ba_prefit_accumulate(P, Q, S, lambda);
+            ba_reduce_system(P, Q, S, npair + 2 * n + 1);
             ba_load_system(P, S, n);                               // S.A = S, S.g = r
             BA_TICK(BA_PH_PF_SYSTEM);
             if (tid == 0) {
-                const double c0 = P.fin[npair + 2 * n];
+                const double c0 = ba_fresh(P.fin)[npair + 2 * n];
                 if (ctl->pcost < 0.0) ctl->pf_cost0 = c0;
                 ctl->pcost = c0;
                 ctl->flag = 1;
             }
             for (int e = tid; e < n * n; e += nt) {
                 const int i = e / n, j = e - i * n;
-                S.L[e] = S.A[e] + (i == j ? lambda * P.fin[npair + n + i] : 0.0);
+                S.L[e] = S.A[e] + (i == j ? lambda * ba_fresh(P.fin)[npair + n + i] : 0.0);
             }
             __syncthreads();
             const bool pd = ba_chol_factor(S.L, n, &ctl->flag);
@@ -1165,7 +1218,7 @@ BA_DEV void ba_solve_body(const BAParams& P, unsigned char* smem) {
             }
             __syncthreads();
             BA_TICK(BA_PH_PF_SOLVE);
-            v3[0] = ba_prefit_backsub(P, S, lambda, scratch); v3[1] = 0.0; v3[2] = 0.0;
+            v3[0] = ba_prefit_backsub(P, Q, S, lambda, scratch); v3[1] = 0.0; v3[2] = 0.0;
             ba_grid_sum3(P, S, slot, v3, tot); slot ^= 1;
             BA_TICK(BA_PH_PF_TRIAL);
             const double cost = ctl->pcost, cost_new = tot[0];
@@ -1173,10 +1226,14 @@ BA_DEV void ba_solve_body(const BAParams& P, unsigned char* smem) {
             __syncthreads();
             if (accept) {
                 for (int e = tid; e < C * 12; e += nt) S.Rt[e] = S.Rt_new[e];
-                const int lt = ba_local_tiles(ctl->ntiles);
+                const int lt = ba_local_tiles(ctl);
                 for (int i = tid; i < lt * BA_TILE; i += nt) {
-                    const int p = ba_point_of(i);
-                    if (p < ctl->m && P.valid[p]) { P.X[3 * p] = P.Xnew[3 * p]; P.X[3 * p + 1] = P.Xnew[3 * p + 1]; P.X[3 * p + 2] = P.Xnew[3 * p + 2]; }
+                    const int p = ba_point_of(S.ctl, i);
+                    if (p < ctl->m && ba_fresh(P.valid)[p]) {
+                        double* X = ba_fresh(P.X);
+                        const double* Xn = ba_fresh(P.Xnew);
+                        X[3 * p] = Xn[3 * p]; X[3 * p + 1] = Xn[3 * p + 1]; X[3 * p + 2] = Xn[3 * p + 2];
+                    }
                 }
                 if (tid == 0) {
                     const double rel = (cost - cost_new) / fmax(cost, 1e-300);
@@ -1209,31 +1266,31 @@ BA_DEV void ba_solve_body(const BAParams& P, unsigned char* smem) {
     // ---- polish: trf_no_bounds -----------------------------------------------------------------------------------
     // linearize at x
     BA_TICK(BA_PH_SETUP);
-    ba_make_columns(P, S);
-    ba_polish_accumulate(P, S);
-    ba_reduce_system(P, S, npair + n + 2);
+    ba_make_columns(P, Q, S);
+    ba_polish_accumulate(P, Q, S);
+    ba_reduce_system(P, Q, S, npair + n + 2);
     ba_load_system(P, S, n);
     BA_TICK(BA_PH_LINEARIZE);
     ba_tridiagonalise(S, n);
     BA_TICK(BA_PH_TRIDIAG);
     if (tid == 0) {
-        ctl->cost = P.fin[npair + n]; ctl->finite = P.fin[npair + n + 1] == 0.0;
-        if (!P.prefit) ctl->cost_initial = ctl->cost;
+        ctl->cost = ba_fresh(P.fin)[npair + n]; ctl->finite = ba_fresh(P.fin)[npair + n + 1] == 0.0;
+        if (!Q.prefit) ctl->cost_initial = ctl->cost;
         ctl->nfev = 1; ctl->njev = 1;
-        double D = P.prefit ? BA_POLISH_RADIUS : ba_norm2_serial(S.x, nf);     // after the prefit the start is already close (ba.cu)
+        double D = Q.prefit ? BA_POLISH_RADIUS : ba_norm2_serial(S.x, nf);     // after the prefit the start is already close (ba.cu)
         if (D == 0.0) D = 1.0;
         ctl->Delta = D; ctl->alpha = 0.0; ctl->iteration = 0; ctl->termination = -99;
         if (!ctl->finite) ctl->termination = -1;
     }
     __syncthreads();
-    const int max_nfev = P.max_nfev > 0 ? P.max_nfev : nf * 100;
+    const int max_nfev = Q.max_nfev > 0 ? Q.max_nfev : nf * 100;
     while (ctl->termination == -99) {
         __syncthreads();                                           // everybody has evaluated the loop condition
         if (tid == 0) {
             double gn = 0.0;
             for (int i = 0; i < n; ++i) gn = fmax(gn, fabs(S.g[i]));
             ctl->g_norm = gn;
-            if (gn < P.gtol) ctl->termination = 1;
+            if (gn < Q.gtol) ctl->termination = 1;
             ctl->go = (ctl->termination == -99 && ctl->nfev != max_nfev) ? 1 : 0;
             ctl->actual = -1.0; ctl->accepted = 0;
         }
@@ -1251,7 +1308,7 @@ BA_DEV void ba_solve_body(const BAParams& P, unsigned char* smem) {
             __syncthreads();
             for (int c = tid; c < C; c += nt) ba_pose_from_x(S.x_new, c, S.Rt_new + 12 * c);
             __syncthreads();
-            ba_cost_pass(P, S, S.Rt_new, false, scratch, v3);
+            ba_cost_pass(P, Q, S, S.Rt_new, false, scratch, v3);
             ba_grid_sum3(P, S, slot, v3, tot); slot ^= 1;
             BA_TICK(BA_PH_TRIAL);
             if (tid == 0) {
@@ -1271,8 +1328,8 @@ BA_DEV void ba_solve_body(const BAParams& P, unsigned char* smem) {
                     if (ratio < 0.25) Delta_new = 0.25 * step_h_norm;
                     else if (ratio > 0.75 && step_h_norm > 0.95 * ctl->Delta) Delta_new = ctl->Delta * 2.0;
                     const double x_norm = ba_norm2_serial(S.x, nf);   // check_termination
-                    const bool ftol_ok = actual < P.ftol * ctl->cost && ratio > 0.25;
-                    const bool xtol_ok = step_h_norm < P.xtol * (P.xtol + x_norm);
+                    const bool ftol_ok = actual < Q.ftol * ctl->cost && ratio > 0.25;
+                    const bool xtol_ok = step_h_norm < Q.xtol * (Q.xtol + x_norm);
                     if (ftol_ok && xtol_ok) ctl->termination = 4;
                     else if (ftol_ok) ctl->termination = 2;
                     else if (xtol_ok) ctl->termination = 3;
@@ -1288,14 +1345,14 @@ BA_DEV void ba_solve_body(const BAParams& P, unsigned char* smem) {
             for (int e = tid; e < C * 12; e += nt) S.Rt[e] = S.Rt_new[e];
             __syncthreads();
             BA_TICK(BA_PH_SETUP);
-            ba_make_columns(P, S);
-            ba_polish_accumulate(P, S);
-            ba_reduce_system(P, S, npair + n + 2);
+            ba_make_columns(P, Q, S);
+            ba_polish_accumulate(P, Q, S);
+            ba_reduce_system(P, Q, S, npair + n + 2);
             ba_load_system(P, S, n);
             BA_TICK(BA_PH_LINEARIZE);
             ba_tridiagonalise(S, n);
             BA_TICK(BA_PH_TRIDIAG);
-            if (tid == 0) { ctl->cost = P.fin[npair + n]; ctl->finite = P.fin[npair + n + 1] == 0.0; ctl->njev += 1; }
+            if (tid == 0) { ctl->cost = ba_fresh(P.fin)[npair + n]; ctl->finite = ba_fresh(P.fin)[npair + n + 1] == 0.0; ctl->njev += 1; }
         }
         if (tid == 0) ctl->iteration += 1;
         __syncthreads();
@@ -1309,7 +1366,7 @@ BA_DEV void ba_solve_body(const BAParams& P, unsigned char* smem) {
     __syncthreads();
 
     // ---- result (helpers.py:290) -----------------------------------------------------------------------------------
-    if (blockIdx.x == 0) {
+    if (ctl->cta == 0) {
         for (int c = tid; c < C; c += nt) {
             double Rt[12];
             ba_pose_from_x(S.x, c, Rt);
@@ -1328,3 +1385,4 @@ BA_DEV void ba_solve_body(const BAParams& P, unsigned char* smem) {
         }
     }
 }
+BA_DEV void ba_solve_body(const BAParams& P, unsigned char* smem) { ba_solve_body(P, P, smem); }
