@@ -207,13 +207,41 @@ MOCAP_API int mocap_reprojection_errors_host(mocap_ctx* ctx, const double* obs, 
  * (index.py:229-270): per adjacent camera pair a fundamental matrix from the common observations,
  * E = K1^T F K0 (cv.sfm.essentialFromFundamental with the intrinsics of cameras 0 and 1), the four
  * motions of cv.sfm.motionFromEssential, the reference's cheirality vote and the pose chain.  The
- * reference's F comes from a randomised cv.findFundamentalMat(FM_RANSAC); here F is a deterministic
+ * reference's F comes from cv.findFundamentalMat(FM_RANSAC) (seeded, repeatable); here F is a
  * normalised 8-point estimate re-fitted twice on its 1 px Sampson inliers, or -- F_given != NULL --
  * supplied by the caller (double [n_cam-1][9], x2^T F x1 = 0).  HOST pointers: obs/mask as for
  * mocap_bundle_adjust_host; R [n_cam][9], t [n_cam][3] out; F_used [n_cam-1][9] and votes
  * [n_cam-1][4] (points in front of the cameras per candidate) may be NULL. */
 MOCAP_API int mocap_calibrate_init_host(mocap_ctx* ctx, const double* obs, const uint8_t* mask, int n_points,
                               const double* F_given, double* R, double* t, double* F_used, int* votes);
+
+/* Robust form of the above: each pair's F comes from RANSAC, as the reference's cv.findFundamentalMat(FM_RANSAC,
+ * 1 px, 0.99999) does (index.py:246), so that mismatched points (a stray reflection recorded in capture-points mode)
+ * do not pull the fit.  For all C-1 pairs at once, on the device: `hypotheses` 7-point samples per pair drawn from
+ * a counter-based hash of (seed, pair, hypothesis) -- the result does not depend on the launch geometry, and is
+ * repeatable for a given seed -- every model scored with cv2's fundamental-matrix error (the larger squared
+ * distance to the two epipolar lines) against threshold_px^2, and per pair the model with the most inliers (ties:
+ * the lowest hypothesis, then root).  The normalised 8-point fit and its Sampson re-selection rounds (at
+ * threshold_px) then start from that model's inliers instead of from all points; E, the cheirality vote (over all
+ * common observations, as index.py:253-257) and the chain are those of mocap_calibrate_init_host.  cv2's sample
+ * sequence is not replayed: parity is defined downstream of F.  HOST pointers; opt NULL = defaults; R, t, F_used,
+ * votes as above; inliers uint8 [n_points][n_cam-1] (may be NULL): 1 where the point is in the pair's final fit
+ * set, 0 elsewhere and where the frame is not common to the pair.  Bad options, or a pair with fewer than 8 common
+ * observations, return MOCAP_EINVAL before anything is launched. */
+typedef struct mocap_ransac_options {
+    double   threshold_px;   /* 1.0 (index.py:246)                              */
+    int      hypotheses;     /* 2048 per pair, 1 .. 65536                        */
+    uint64_t seed;           /* 0                                                */
+} mocap_ransac_options;
+MOCAP_API void mocap_ransac_default_options(mocap_ransac_options* opt);
+MOCAP_API int  mocap_calibrate_init_ransac_host(mocap_ctx* ctx, const double* obs, const uint8_t* mask, int n_points,
+                                      const mocap_ransac_options* opt, double* R, double* t, double* F_used,
+                                      int* votes, uint8_t* inliers);
+/* The RANSAC stage of the above alone: per adjacent pair the winning model F [n_cam-1][9] (unit Frobenius norm,
+ * x2^T F x1 = 0) and its inliers uint8 [n_points][n_cam-1] (may be NULL) at threshold_px, before any refinement.
+ * Three kernel launches whatever the number of cameras.  Needs no intrinsics.  HOST pointers. */
+MOCAP_API int  mocap_fundamental_ransac_host(mocap_ctx* ctx, const double* obs, const uint8_t* mask, int n_points,
+                                   const mocap_ransac_options* opt, double* F, uint8_t* inliers);
 
 /* S4 -- replaces bundle_adjustment (helpers.py:244-290): robust (Cauchy) trust-region
  * least squares over the poses of cameras 1..C-1 (rotation vector + translation;

@@ -37,6 +37,10 @@ class BAReport(C.Structure):
                 ("n_tr_newton", C.c_int), ("phase_ms", C.c_float * 8)]
 
 
+class RansacOptions(C.Structure):
+    _fields_ = [("threshold_px", C.c_double), ("hypotheses", C.c_int), ("seed", C.c_uint64)]
+
+
 class BAProblem(C.Structure):
     _fields_ = [("obs", C.c_void_p), ("mask", C.c_void_p), ("n_points_max", C.c_int), ("n_points", C.c_void_p),
                 ("R", C.c_void_p), ("t", C.c_void_p), ("report", C.c_void_p)]
@@ -68,6 +72,9 @@ SYMBOLS = {
     "mocap_triangulate_host": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, _P]),
     "mocap_reprojection_errors_host": (C.c_int, [_P, _P, _P, _P, C.c_int, _P, _P]),
     "mocap_calibrate_init_host": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, _P, _P, _P]),
+    "mocap_ransac_default_options": (None, [C.POINTER(RansacOptions)]),
+    "mocap_calibrate_init_ransac_host": (C.c_int, [_P, _P, _P, C.c_int, C.POINTER(RansacOptions), _P, _P, _P, _P, _P]),
+    "mocap_fundamental_ransac_host": (C.c_int, [_P, _P, _P, C.c_int, C.POINTER(RansacOptions), _P, _P]),
     "mocap_ba_default_options": (None, [C.POINTER(BAOptions)]),
     "mocap_bundle_adjust_host": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, C.POINTER(BAOptions), C.POINTER(BAReport)]),
     "mocap_bundle_adjust_dev": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, _P, C.POINTER(BAOptions), _P]),

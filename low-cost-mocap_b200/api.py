@@ -21,7 +21,7 @@ import threading
 import numpy as np
 
 from . import _lib
-from ._lib import MocapError, Config, BAOptions, BAProblem, BAReport, check
+from ._lib import MocapError, Config, BAOptions, BAProblem, BAReport, RansacOptions, check
 
 THRESHOLD = 51   # cv.threshold(grey, 255*0.2, 255, THRESH_BINARY) on uint8 == pix > 51 (helpers.py:146)
 
@@ -378,17 +378,50 @@ class MocapContext:
         self._check(self.lib.mocap_reprojection_errors_host(self.h, _np_ptr(obs), _np_ptr(mask), _np_ptr(X), F, _np_ptr(err), _np_ptr(valid)))
         return err, valid
 
-    def calibrate_init(self, obs, mask, F_given=None):
-        """Chain of relative poses from 2D tracks (index.py:229-270).  Returns (poses, F_used [C-1,3,3], votes [C-1,4])."""
+    def _ransac_options(self, threshold, hypotheses, seed):
+        opt = RansacOptions()
+        self.lib.mocap_ransac_default_options(C.byref(opt))
+        opt.threshold_px, opt.hypotheses, opt.seed = float(threshold), int(hypotheses), int(seed)
+        return opt
+
+    def calibrate_init(self, obs, mask, F_given=None, method="8point", threshold=1.0, hypotheses=2048, seed=0):
+        """Chain of relative poses from 2D tracks (index.py:229-270).  Returns (poses, F_used [C-1,3,3], votes [C-1,4]).
+
+        ``method="8point"``: each pair's F is a normalised 8-point fit to all common observations, re-fitted on its
+        1 px Sampson inliers (or ``F_given``).  ``method="ransac"``: the fit starts from the inliers of a RANSAC model
+        (``hypotheses`` 7-point samples per pair from ``seed``, inliers within ``threshold`` px), which mismatched
+        points do not pull; the return then also holds the per-pair inlier masks, uint8 [F, C-1]."""
         obs = np.ascontiguousarray(obs, dtype=np.float64)
         mask = np.ascontiguousarray(mask, dtype=np.uint8)
         Cn = self.n_cam
         R = np.empty((Cn, 3, 3)); t = np.empty((Cn, 3))
         Fu = np.empty((Cn - 1, 3, 3)); votes = np.empty((Cn - 1, 4), dtype=np.int32)
+        if method == "ransac":
+            if F_given is not None:
+                raise ValueError("calibrate_init: F_given and method='ransac' exclude each other")
+            inl = np.empty((obs.shape[0], Cn - 1), dtype=np.uint8)
+            opt = self._ransac_options(threshold, hypotheses, seed)
+            self._check(self.lib.mocap_calibrate_init_ransac_host(self.h, _np_ptr(obs), _np_ptr(mask), obs.shape[0], C.byref(opt),
+                                                                  _np_ptr(R), _np_ptr(t), _np_ptr(Fu), _np_ptr(votes), _np_ptr(inl)))
+            return [{"R": R[i].copy(), "t": t[i].copy()} for i in range(Cn)], Fu, votes, inl
+        if method != "8point":
+            raise ValueError(f"calibrate_init: unknown method {method!r} (expected '8point' or 'ransac')")
         Fg = None if F_given is None else np.ascontiguousarray(np.asarray(F_given, dtype=np.float64).reshape(Cn - 1, 3, 3))
         self._check(self.lib.mocap_calibrate_init_host(self.h, _np_ptr(obs), _np_ptr(mask), obs.shape[0], _np_ptr(Fg),
                                                        _np_ptr(R), _np_ptr(t), _np_ptr(Fu), _np_ptr(votes)))
         return [{"R": R[i].copy(), "t": t[i].copy()} for i in range(Cn)], Fu, votes
+
+    def fundamental_ransac(self, obs, mask, threshold=1.0, hypotheses=2048, seed=0):
+        """The RANSAC stage of ``calibrate_init(method="ransac")`` alone: per adjacent pair the winning 7-point model
+        and its inliers within ``threshold`` px, before any refinement.  Returns (F [C-1,3,3], inliers uint8 [F, C-1])."""
+        obs = np.ascontiguousarray(obs, dtype=np.float64)
+        mask = np.ascontiguousarray(mask, dtype=np.uint8)
+        Cn = self.n_cam
+        F = np.empty((Cn - 1, 3, 3)); inl = np.empty((obs.shape[0], Cn - 1), dtype=np.uint8)
+        opt = self._ransac_options(threshold, hypotheses, seed)
+        self._check(self.lib.mocap_fundamental_ransac_host(self.h, _np_ptr(obs), _np_ptr(mask), obs.shape[0], C.byref(opt),
+                                                           _np_ptr(F), _np_ptr(inl)))
+        return F, inl
 
     def ba_residuals(self, obs, mask, poses):
         obs = np.ascontiguousarray(obs, dtype=np.float64)
@@ -629,10 +662,12 @@ def bundle_adjustment(image_points, camera_poses, socketio, session=None):
     return out
 
 
-def calculate_camera_poses(image_points, socketio=None, session=None):
+def calculate_camera_poses(image_points, socketio=None, session=None, robust=False):
     """The computation of the reference's ``calculate-camera-pose`` handler (index.py:229-277): cold-start
     chain of relative poses, then bundle adjustment.  ``image_points`` is the (F, C, 2) list the UI sends
-    (``data["cameraPoints"]``) with ``None`` for missing views.  Returns the list of {"R", "t"}."""
+    (``data["cameraPoints"]``) with ``None`` for missing views.  ``robust=True`` starts the chain from RANSAC
+    fundamental matrices (``MocapContext.calibrate_init(method="ransac")``), which mismatched points -- a stray
+    reflection recorded as a camera's first point -- do not pull.  Returns the list of {"R", "t"}."""
     s = session or MocapSession.default()
     obs, mask = _split_observations(image_points)
     n_cam = obs.shape[1]
@@ -640,7 +675,7 @@ def calculate_camera_poses(image_points, socketio=None, session=None):
         ctx = s.ctx(n_cam)
         ident = [{"R": np.eye(3), "t": np.zeros(3)} for _ in range(n_cam)]
         ctx.set_cameras(s.intrinsics[:n_cam], ident)
-        start, _, _ = ctx.calibrate_init(obs, mask)
+        start = ctx.calibrate_init(obs, mask, method="ransac" if robust else "8point")[0]
         ctx.set_cameras(s.intrinsics[:n_cam], start)
         out, _ = ctx.bundle_adjust(obs, mask, start)
     if socketio is not None:

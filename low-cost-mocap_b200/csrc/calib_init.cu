@@ -6,9 +6,10 @@
 // (R, t) of cv.sfm.motionFromEssential, the cheirality vote with the reference's own (odd) counting rule
 // (index.py:253-262), and the pose chain (index.py:264-265).  bundle_adjustment then refines the chain.
 //
-// The reference estimates F with cv.findFundamentalMat(FM_RANSAC, 1 px, 0.99999), which is randomised
-// and returns a 7-point minimal-sample model; this implementation is deterministic instead: normalised
-// 8-point over all common observations, two rounds of re-estimation on the Sampson inliers (1 px), rank
+// The reference estimates F with cv.findFundamentalMat(FM_RANSAC, 1 px, 0.99999), whose generator starts from a
+// fixed state (repeatable, but its sample sequence is not replayed here) and which returns a 7-point minimal-sample
+// model.  This file's estimator: normalised 8-point over all common observations -- or, for the robust method
+// (calib_ransac.cu), over the inliers of a RANSAC model -- two rounds of re-estimation on the Sampson inliers, rank
 // 2 enforced.  Parity is therefore defined downstream of F (SURVEY.md section 8(c)): given the same F the
 // chosen (R, t) must be the reference's, and end to end the adjusted rig must be at least as good.
 //
@@ -161,9 +162,13 @@ void motion_from_essential(const double E[9], double Rs[4][9], double ts[4][3]) 
 
 // One adjacent pair.  p1/p2: device [n][2] common observations.  F_in (host, 9) may be given (then no
 // estimation); F_out receives the matrix used.  prev_R/prev_t: accumulated pose of the first camera.
+// init_inl (host, n; NULL = all points) is the set the first 8-point fit uses -- a set of fewer than 8 falls back to
+// all points; thr2 is the squared Sampson threshold of the re-selection rounds; inl_out (host, n; may be NULL)
+// receives the final inlier set of the rounds.
 static int pair_motion(mocap_ctx* ctx, const double* d_p1, const double* d_p2, uint8_t* d_inl, double* d_work, int n,
                        const double* F_in, double* F_out, const double* K0, const double* K1, const double* prev_R,
-                       const double* prev_t, double* R_rel, double* t_rel, int* votes) {
+                       const double* prev_t, double* R_rel, double* t_rel, int* votes, const uint8_t* init_inl,
+                       double thr2, uint8_t* inl_out) {
     cudaStream_t s = ctx->stream;
     double F[9];
     if (F_in) memcpy(F, F_in, sizeof(F));
@@ -174,6 +179,11 @@ static int pair_motion(mocap_ctx* ctx, const double* d_p1, const double* d_p2, u
         CUDA_TRY(ctx, cudaMemcpyAsync(h2.data(), d_p2, h2.size() * 8, cudaMemcpyDeviceToHost, s));
         CUDA_TRY(ctx, cudaStreamSynchronize(s));
         std::vector<uint8_t> inl(n, 1);
+        if (init_inl) {
+            int m0 = 0;
+            for (int i = 0; i < n; ++i) m0 += init_inl[i] ? 1 : 0;
+            if (m0 >= 8) for (int i = 0; i < n; ++i) inl[i] = init_inl[i] ? 1 : 0;
+        }
         for (int round = 0; round < 3; ++round) {
             double T1[3], T2[3];
             for (int side = 0; side < 2; ++side) {
@@ -220,11 +230,11 @@ static int pair_motion(mocap_ctx* ctx, const double* d_p1, const double* d_p2, u
             double nf = 0; for (int i = 0; i < 9; ++i) nf += F[i] * F[i];
             nf = sqrt(nf); if (nf > 0) for (int i = 0; i < 9; ++i) F[i] /= nf;
             if (round == 2) break;
-            // Sampson inliers at 1 px (the reference's RANSAC threshold, index.py:246)
+            // Sampson inliers at thr2 (1 px: the reference's RANSAC threshold, index.py:246)
             int* d_cnt = reinterpret_cast<int*>(d_work + 64);
             CUDA_TRY(ctx, cudaMemcpyAsync(d_work + 54, F, sizeof(F), cudaMemcpyHostToDevice, s));
             CUDA_TRY(ctx, cudaMemsetAsync(d_cnt, 0, sizeof(int), s));
-            k_sampson_inliers<<<(n + 255) / 256, 256, 0, s>>>(d_p1, d_p2, n, d_work + 54, 1.0, d_inl, d_cnt);
+            k_sampson_inliers<<<(n + 255) / 256, 256, 0, s>>>(d_p1, d_p2, n, d_work + 54, thr2, d_inl, d_cnt);
             CUDA_TRY(ctx, cudaGetLastError());
             ctx->launches += 1;
             int cnt = 0;
@@ -233,6 +243,7 @@ static int pair_motion(mocap_ctx* ctx, const double* d_p1, const double* d_p2, u
             CUDA_TRY(ctx, cudaStreamSynchronize(s));
             if (cnt < 8 || cnt == n) { if (cnt < 8) std::fill(inl.begin(), inl.end(), 1); if (cnt == n && round > 0) break; }
         }
+        if (inl_out) memcpy(inl_out, inl.data(), n);
     }
     if (F_out) memcpy(F_out, F, sizeof(F));
     // E = K1^T F K0 (libmv EssentialFromFundamental(F, K1=first arg, K2=second arg) = K2^T F K1; index.py:247 passes K[0], K[1])
@@ -277,12 +288,12 @@ static int pair_motion(mocap_ctx* ctx, const double* d_p1, const double* d_p2, u
     return MOCAP_OK;
 }
 
-extern "C" int mocap_calibrate_init_host(mocap_ctx* ctx, const double* obs, const uint8_t* mask, int n_points,
-                                         const double* F_given, double* R, double* t, double* F_used, int* votes) {
-    if (!ctx) return MOCAP_EINVAL;
+// The pose chain of index.py:235-265 over all adjacent pairs (see pair_motion).  init_inl (host; may be NULL) holds
+// each pair's initial fit set over its common observations in frame order, pair after pair; inl_out (host,
+// [n_points][C-1]; may be NULL) receives each pair's final inlier set, 0 where the frame is not common to the pair.
+int calibrate_chain(mocap_ctx* ctx, const double* obs, const uint8_t* mask, int n_points, const double* F_given,
+                    const uint8_t* init_inl, double thr2, double* R, double* t, double* F_used, int* votes, uint8_t* inl_out) {
     const int C = ctx->cfg.n_cam;
-    if (!obs || !mask || !R || !t || n_points < 8 || C < 2) return mocap_fail(ctx, MOCAP_EINVAL, "mocap_calibrate_init_host: bad argument");
-    if (!ctx->cameras_set) return mocap_fail(ctx, MOCAP_ESTATE, "mocap_set_cameras has not been called (intrinsics are needed)");
     CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));
     const size_t n = (size_t)n_points;
     int st = ensure_scratch(ctx, n * 2 * 8 * 2 + n + 4096);
@@ -298,6 +309,9 @@ extern "C" int mocap_calibrate_init_host(mocap_ctx* ctx, const double* obs, cons
     const double* K0 = ctx->h_tables.Kmat[0];
     const double* K1 = ctx->h_tables.Kmat[C > 1 ? 1 : 0];
     std::vector<double> h1, h2;
+    std::vector<uint8_t> pair_inl(inl_out ? n : 0);
+    size_t init_off = 0;
+    if (inl_out) memset(inl_out, 0, n * (C - 1));
     for (int c = 0; c + 1 < C; ++c) {
         h1.clear(); h2.clear();
         for (int f = 0; f < n_points; ++f)
@@ -313,8 +327,13 @@ extern "C" int mocap_calibrate_init_host(mocap_ctx* ctx, const double* obs, cons
         CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
         double R_rel[9], t_rel[3];
         st = pair_motion(ctx, d_p1, d_p2, d_inl, d_work, m, F_given ? F_given + 9 * c : nullptr, F_used ? F_used + 9 * c : nullptr, K0, K1,
-                         R + 9 * c, t + 3 * c, R_rel, t_rel, votes ? votes + 4 * c : nullptr);
+                         R + 9 * c, t + 3 * c, R_rel, t_rel, votes ? votes + 4 * c : nullptr, init_inl ? init_inl + init_off : nullptr,
+                         thr2, inl_out ? pair_inl.data() : nullptr);
         if (st) return st;
+        init_off += (size_t)m;
+        if (inl_out)
+            for (int f = 0, k = 0; f < n_points; ++f)
+                if (mask[(size_t)f * C + c] && mask[(size_t)f * C + c + 1]) inl_out[(size_t)f * (C - 1) + c] = pair_inl[k++];
         // index.py:264-265: R = R_rel @ R_prev ; t = t_prev + R_prev @ t_rel
         mat3mul(R_rel, R + 9 * c, R + 9 * (c + 1));
         for (int i = 0; i < 3; ++i) {
@@ -324,4 +343,13 @@ extern "C" int mocap_calibrate_init_host(mocap_ctx* ctx, const double* obs, cons
         }
     }
     return MOCAP_OK;
+}
+
+extern "C" int mocap_calibrate_init_host(mocap_ctx* ctx, const double* obs, const uint8_t* mask, int n_points,
+                                         const double* F_given, double* R, double* t, double* F_used, int* votes) {
+    if (!ctx) return MOCAP_EINVAL;
+    const int C = ctx->cfg.n_cam;
+    if (!obs || !mask || !R || !t || n_points < 8 || C < 2) return mocap_fail(ctx, MOCAP_EINVAL, "mocap_calibrate_init_host: bad argument");
+    if (!ctx->cameras_set) return mocap_fail(ctx, MOCAP_ESTATE, "mocap_set_cameras has not been called (intrinsics are needed)");
+    return calibrate_chain(ctx, obs, mask, n_points, F_given, nullptr, 1.0, R, t, F_used, votes, nullptr);
 }

@@ -117,3 +117,7 @@ int launch_pipeline_tma(mocap_ctx* ctx, const uint8_t* frames, int n_sets, int t
 int launch_pipeline_fused(mocap_ctx* ctx, const uint8_t* frames, int n_sets, int threshold,
                           double* obj, double* err, int32_t* n_obj, int32_t* set_flags, int channels = 1);
 int timing_flush(mocap_ctx* ctx);
+// cold-start pose chain (calib_init.cu): per adjacent pair an 8-point F started from init_inl (NULL = all common
+// observations) and re-fitted on its Sampson inliers at thr2, E, the cheirality vote and the chain
+int calibrate_chain(mocap_ctx* ctx, const double* obs, const uint8_t* mask, int n_points, const double* F_given,
+                    const uint8_t* init_inl, double thr2, double* R, double* t, double* F_used, int* votes, uint8_t* inl_out);
