@@ -342,6 +342,25 @@ MOCAP_API int  mocap_bundle_adjust_batch_dev(mocap_ctx* ctx, const mocap_ba_prob
 MOCAP_API int  mocap_tracks_to_observations_dev(mocap_ctx* ctx, const int32_t* track_xy, const int32_t* n_obj,
                                       const double* err, int n_frame_sets, double max_err, double* obs,
                                       uint8_t* mask, int32_t* n_points, int capacity);
+/* Per-view screening of explicit correspondences against poses (rule in DESIGN section 5): for each track, the
+ * 2-view DLT point of every pair of its views in mask_in, the pair whose point the most views reproject to within
+ * threshold_px wins (ties to the earlier pair), its supporting views are re-triangulated and the views within
+ * threshold_px of that point are kept if they are >= 2 and all pass against their own DLT point; otherwise the row is
+ * emptied (the track leaves the adjustment).  Rows with fewer than two views are copied unchanged.  The arithmetic is
+ * that of the bundle adjustment's residual.  Screen again from the caller's ORIGINAL mask after each adjustment, so
+ * that a view dropped under poor poses can come back.  obs double [n_points_max][n_cam][2], mask_in / mask_out uint8
+ * [n_points_max][n_cam] (rows past *n_points are left untouched), R [n_cam][9], t [n_cam][3] the CURRENT poses (e.g.
+ * the buffers mocap_bundle_adjust_dev updates), stats int32 [4] = views in, views kept, views dropped, rows emptied.
+ * DEVICE pointers, one launch, never synchronises; n_points may be NULL (= n_points_max); stats may be NULL.  A
+ * threshold_px that is <= 0 or not finite, a NULL obs / mask / R / t / mask_out, or mask_out == mask_in returns
+ * MOCAP_EINVAL before any launch. */
+MOCAP_API int  mocap_screen_observations_dev(mocap_ctx* ctx, const double* obs, const uint8_t* mask_in, int n_points_max,
+                                   const int32_t* n_points, const double* R, const double* t, double threshold_px,
+                                   uint8_t* mask_out, int32_t* stats);
+/* The same with HOST pointers (n_points a host int32, may be NULL); copies inside and synchronises. */
+MOCAP_API int  mocap_screen_observations_host(mocap_ctx* ctx, const double* obs, const uint8_t* mask_in, int n_points_max,
+                                    const int32_t* n_points, const double* R, const double* t, double threshold_px,
+                                    uint8_t* mask_out, int32_t* stats);
 /* residual vector of S4 at explicit poses (helpers.py:264-276); r float [n_points],
  * valid uint8 [n_points]; returns the number of valid residuals in *n_valid. HOST pointers. */
 MOCAP_API int  mocap_ba_residuals_host(mocap_ctx* ctx, const double* obs, const uint8_t* mask, int n_points,

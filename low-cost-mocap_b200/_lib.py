@@ -82,6 +82,8 @@ SYMBOLS = {
     "mocap_bundle_adjust_batch_dev": (C.c_int, [_P, C.POINTER(BAProblem), C.c_int, C.POINTER(BAOptions)]),
     "mocap_tracks_to_observations_dev": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_double, _P, _P, _P, C.c_int]),
     "mocap_pipeline_tracks_dev": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P]),
+    "mocap_screen_observations_dev": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, _P, C.c_double, _P, _P]),
+    "mocap_screen_observations_host": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, _P, C.c_double, _P, _P]),
     "mocap_ba_residuals_host": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, _P, _P, C.POINTER(C.c_int)]),
     "mocap_host_alloc": (C.c_int, [C.POINTER(_P), C.c_uint64]),
     "mocap_host_free": (None, [_P]),

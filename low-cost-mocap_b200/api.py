@@ -319,6 +319,66 @@ class MocapContext:
         self._check(self.lib.mocap_bundle_adjust_batch_dev(self.h, arr, len(problems), C.byref(opt)))
         return reports
 
+    def screen_observations_dev(self, obs, mask, R, t, threshold_px, n_points=None, out=None):
+        """Per-view screen of explicit correspondences against the current poses (mocap_screen_observations_dev, rule in
+        DESIGN section 5): obs f64 [P, C, 2], mask uint8 [P, C] (the caller's ORIGINAL mask), R f64 [C, 3, 3], t f64
+        [C, 3] cuda tensors, n_points an int32 cuda tensor [1] or None.  One launch, no synchronisation.  Returns dict
+        mask uint8 [P, C] (rows past n_points untouched), stats int32 [4] = views in, kept, dropped, rows emptied."""
+        torch = _torch()
+        if out is None:
+            out = {"mask": torch.empty_like(mask), "stats": torch.empty((4,), dtype=torch.int32, device=mask.device)}
+        self.use_current_stream()
+        self._check(self.lib.mocap_screen_observations_dev(self.h, _ptr(obs), _ptr(mask), obs.shape[0], _ptr(n_points), _ptr(R), _ptr(t),
+                                                           float(threshold_px), _ptr(out["mask"]), _ptr(out["stats"])))
+        return out
+
+    def screen_observations(self, obs, mask, poses, threshold_px):
+        """The same on host arrays: obs float64 [P, C, 2], mask uint8 [P, C], poses a list of {"R", "t"}.  Returns dict
+        mask uint8 [P, C], stats int32 [4]."""
+        obs = np.ascontiguousarray(obs, dtype=np.float64)
+        mask = np.ascontiguousarray(mask, dtype=np.uint8)
+        R = np.ascontiguousarray(np.stack([np.asarray(p["R"], dtype=np.float64).reshape(3, 3) for p in poses]))
+        t = np.ascontiguousarray(np.stack([np.asarray(p["t"], dtype=np.float64).reshape(3) for p in poses]))
+        out = np.zeros_like(mask)
+        stats = np.zeros((4,), dtype=np.int32)
+        self._check(self.lib.mocap_screen_observations_host(self.h, _np_ptr(obs), _np_ptr(mask), obs.shape[0], None, _np_ptr(R), _np_ptr(t),
+                                                            float(threshold_px), _np_ptr(out), _np_ptr(stats)))
+        return {"mask": out, "stats": stats}
+
+    def bundle_adjust_screened(self, obs, mask, poses, threshold_px, rounds=2, first_mask=None, **ba_kw):
+        """Bundle adjustment that screens mismatched views out between rounds, all on the device with no synchronisation
+        until the final copy-out: ``bundle_adjust_dev(first_mask)``, then ``rounds`` times [screen the ORIGINAL mask at
+        the current poses -> ``bundle_adjust_dev(screened mask)``].  A view dropped under early poses can come back once
+        they improve.  ``first_mask`` (None: ``mask``) is what the first solve sees: the mismatched views a solve keeps
+        pull the poses so far that the first screen would lose most good views with them (INTEGRATION.md section 2), so
+        a cleaner first guess -- e.g. the views that are RANSAC inliers with a neighbouring camera -- helps.  obs / mask
+        host arrays, poses a list of {"R", "t"}; ``ba_kw`` go to every solve.  Returns (poses, report of the last solve,
+        kept mask uint8 [P, C] -- the first solve's mask when rounds == 0)."""
+        torch = _torch()
+        if int(rounds) != rounds or rounds < 0:
+            raise ValueError(f"bundle_adjust_screened: rounds must be a non-negative integer (got {rounds!r})")
+        if not (threshold_px > 0 and np.isfinite(threshold_px)):
+            raise MocapError(-1, f"bundle_adjust_screened: threshold_px must be positive and finite (got {threshold_px})")
+        dev = self.torch_device
+        d_obs = torch.from_numpy(np.ascontiguousarray(obs, dtype=np.float64)).to(dev)
+        d_mask = torch.from_numpy(np.ascontiguousarray(mask, dtype=np.uint8)).to(dev)
+        R = torch.from_numpy(np.stack([np.asarray(p["R"], dtype=np.float64).reshape(3, 3) for p in poses])).to(dev)
+        t = torch.from_numpy(np.stack([np.asarray(p["t"], dtype=np.float64).reshape(3) for p in poses])).to(dev)
+        d_first = d_mask if first_mask is None else torch.from_numpy(np.ascontiguousarray(first_mask, dtype=np.uint8)).to(dev)
+        if d_first.shape != d_mask.shape:
+            raise ValueError("bundle_adjust_screened: first_mask must have the shape of mask")
+        screened = {"mask": torch.empty_like(d_mask), "stats": torch.empty((4,), dtype=torch.int32, device=dev)}
+        report = self.bundle_adjust_dev(d_obs, d_first, R, t, **ba_kw)
+        for _ in range(int(rounds)):
+            self.screen_observations_dev(d_obs, d_mask, R, t, threshold_px, out=screened)
+            report = self.bundle_adjust_dev(d_obs, screened["mask"], R, t, report=report, **ba_kw)
+        rep = self.decode_ba_report(report)
+        if rep["status"] == -3:
+            raise MocapError(-1, "bundle_adjust_screened: no point is seen by two cameras")
+        kept = (screened["mask"] if rounds else d_first).cpu().numpy()
+        R, t = R.cpu().numpy(), t.cpu().numpy()
+        return [{"R": R[i].copy(), "t": t[i].copy()} for i in range(self.n_cam)], rep, kept
+
     @staticmethod
     def decode_ba_report(report):
         rep = BAReport.from_buffer_copy(report.cpu().numpy().tobytes())
@@ -662,12 +722,15 @@ def bundle_adjustment(image_points, camera_poses, socketio, session=None):
     return out
 
 
-def calculate_camera_poses(image_points, socketio=None, session=None, robust=False):
+def calculate_camera_poses(image_points, socketio=None, session=None, robust=False, reject_px=None, rounds=2):
     """The computation of the reference's ``calculate-camera-pose`` handler (index.py:229-277): cold-start
     chain of relative poses, then bundle adjustment.  ``image_points`` is the (F, C, 2) list the UI sends
     (``data["cameraPoints"]``) with ``None`` for missing views.  ``robust=True`` starts the chain from RANSAC
     fundamental matrices (``MocapContext.calibrate_init(method="ransac")``), which mismatched points -- a stray
-    reflection recorded as a camera's first point -- do not pull.  Returns the list of {"R", "t"}."""
+    reflection recorded as a camera's first point -- do not pull.  ``reject_px`` (None: every view enters the
+    adjustment, as in the reference) screens views that disagree with their track by more than that many pixels out
+    of the adjustment, ``rounds`` times (``MocapContext.bundle_adjust_screened``; INTEGRATION.md recommends a value).
+    Returns the list of {"R", "t"}."""
     s = session or MocapSession.default()
     obs, mask = _split_observations(image_points)
     n_cam = obs.shape[1]
@@ -675,9 +738,22 @@ def calculate_camera_poses(image_points, socketio=None, session=None, robust=Fal
         ctx = s.ctx(n_cam)
         ident = [{"R": np.eye(3), "t": np.zeros(3)} for _ in range(n_cam)]
         ctx.set_cameras(s.intrinsics[:n_cam], ident)
-        start = ctx.calibrate_init(obs, mask, method="ransac" if robust else "8point")[0]
+        init = ctx.calibrate_init(obs, mask, method="ransac" if robust else "8point")
+        start = init[0]
         ctx.set_cameras(s.intrinsics[:n_cam], start)
-        out, _ = ctx.bundle_adjust(obs, mask, start)
+        if reject_px is None:
+            out, _ = ctx.bundle_adjust(obs, mask, start)
+        else:
+            first = None
+            if robust:
+                # the first solve sees the views that are RANSAC inliers with a neighbouring camera; the screens that
+                # follow start from every view again
+                inl = init[3].astype(bool)
+                near = np.zeros(mask.shape, dtype=bool)
+                near[:, :-1] |= inl
+                near[:, 1:] |= inl
+                first = (mask.astype(bool) & near).astype(np.uint8)
+            out, _, _ = ctx.bundle_adjust_screened(obs, mask, start, reject_px, rounds=rounds, first_mask=first)
     if socketio is not None:
         socketio.emit("camera-pose", {"camera_poses": [{"R": p["R"].tolist(), "t": p["t"].tolist()} for p in out]})
     return out

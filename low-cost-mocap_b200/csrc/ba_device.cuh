@@ -187,16 +187,9 @@ BA_DEV void ba_pose_from_x(const double* x, int c, double Rt[12]) {
     }
 }
 
-// K_k [R|t] summed like the BLAS micro-kernel the reference's numpy call runs (see ba.cu make_P)
-BA_DEV void ba_make_P(const double* Kk, const double* Rt, double P[12]) {
-    for (int i = 0; i < 3; ++i)
-        for (int j = 0; j < 4; ++j) {
-            double acc = DMUL(Kk[3 * i + 0], Rt[j]);
-            acc = DFMA(Kk[3 * i + 1], Rt[4 + j], acc);
-            acc = DFMA(Kk[3 * i + 2], Rt[8 + j], acc);
-            P[4 * i + j] = acc;
-        }
-}
+// K_k [R|t] summed like the BLAS micro-kernel the reference's numpy call runs (geom.cuh; the screen of screen.cuh
+// builds its projection matrices with the same function)
+BA_DEV void ba_make_P(const double* Kk, const double* Rt, double P[12]) { make_P_like_blas(Kk, Rt, P); }
 
 // residual_function of the reference for one point (helpers.py:264-276): DLT with the trial poses, reprojection
 // error like cv.projectPoints, mean in numpy's order.  Camera `cam` (if >= 0) takes the pose colRt instead of its

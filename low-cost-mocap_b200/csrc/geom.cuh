@@ -55,6 +55,18 @@ GEOM_HD void dlt_add_view(Sym4& B, const double* __restrict__ P, double x, doubl
     sym4_add_row(B, b0, b1, b2, b3);
 }
 
+// K_k [R|t] (Kk 3x3, Rt 3x4, both row-major) summed like the BLAS micro-kernel the reference's numpy call runs:
+// fused multiply-adds over the inner index (see ba.cu make_P)
+GEOM_HD void make_P_like_blas(const double* Kk, const double* Rt, double P[12]) {
+    for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < 4; ++j) {
+            double acc = DMUL(Kk[3 * i + 0], Rt[j]);
+            acc = DFMA(Kk[3 * i + 1], Rt[4 + j], acc);
+            acc = DFMA(Kk[3 * i + 2], Rt[8 + j], acc);
+            P[4 * i + j] = acc;
+        }
+}
+
 #define JROT(p, q)                                                                       \
     {                                                                                     \
         const double apq = a[p][q];                                                       \

@@ -2,7 +2,9 @@
 """Wall time of the cold-start calibration: calibrate_init with the 8-point and the RANSAC estimator, the RANSAC stage
 alone (fundamental_ransac: three kernels for all pairs), and calculate_camera_poses(robust=True), at 4, 8 and 16
 cameras x 6400 points (16 x 6400 is BASELINE config 5: 64 markers x 100 frames), 10 % of each camera's observations
-mismatched.  Beside them the CPU time of cv2.findFundamentalMat(FM_RANSAC, 1 px, 0.99999) over the same pairs, the
+mismatched; calculate_camera_poses(robust=True, reject_px=REJECT_PX) beside it, and at 16 cameras the screen kernel
+alone (CUDA events over many launches, each with its stats reset) and one bundle-adjustment solve of the screened
+tracks.  Beside them the CPU time of cv2.findFundamentalMat(FM_RANSAC, 1 px, 0.99999) over the same pairs, the
 reference handler's estimator.  Every entry point synchronises before it returns, so a host clock around each call
 measures it; the variants are alternated and medians reported.  Prints one JSON document (GPU name and power limit
 included); --out also writes it to a file."""
@@ -14,6 +16,7 @@ import cv2
 import torch
 pkg = importlib.import_module("low-cost-mocap_b200")
 synth = pkg.synth
+REJECT_PX = 8.0      # the value INTEGRATION.md recommends for calculate_camera_poses(reject_px=...)
 
 
 def tracks(C, n, frac=0.1, seed=3):
@@ -35,6 +38,40 @@ def cv2_pairs(obs, mask):
         cv2.findFundamentalMat(obs[both, c].astype(np.float32), obs[both, c + 1].astype(np.float32), cv2.FM_RANSAC, 1, 0.99999)
 
 
+def screen_kernel_ms(obs, mask, K, launches=200, solves=10):
+    """Device time of k_screen_observations alone (CUDA events around `launches` back-to-back launches) at the poses
+    of the robust chain's first bundle adjustment, and of one k_ba_solve from the same poses for scale."""
+    C = obs.shape[1]
+    ctx = pkg.MocapContext(C)
+    ctx.set_cameras([K] * C, [{"R": np.eye(3), "t": np.zeros(3)}] * C)
+    chain = ctx.calibrate_init(obs, mask, method="ransac")[0]
+    ctx.set_cameras([K] * C, chain)
+    first, _ = ctx.bundle_adjust(obs, mask, chain)
+    dev = ctx.torch_device
+    d_obs, d_mask = torch.from_numpy(obs).to(dev), torch.from_numpy(mask).to(dev)
+    R0 = torch.from_numpy(np.stack([p["R"] for p in first])).to(dev)
+    t0 = torch.from_numpy(np.stack([p["t"] for p in first])).to(dev)
+    out = ctx.screen_observations_dev(d_obs, d_mask, R0, t0, REJECT_PX)
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(launches):
+        ctx.screen_observations_dev(d_obs, d_mask, R0, t0, REJECT_PX, out=out)
+    e1.record()
+    torch.cuda.synchronize()
+    screen = e0.elapsed_time(e1) / launches
+    R, t = R0.clone(), t0.clone()
+    solve = []
+    for _ in range(solves):
+        R.copy_(R0); t.copy_(t0)
+        e0.record()
+        ctx.bundle_adjust_dev(d_obs, out["mask"], R, t)
+        e1.record()
+        torch.cuda.synchronize()
+        solve.append(e0.elapsed_time(e1))
+    return {"screen_kernel_ms": screen, "launches": launches, "stats": out["stats"].cpu().tolist(),
+            "ba_solve_after_screen_ms_median": float(np.median(solve))}
+
+
 def case(C, n, reps):
     obs, mask, image_points, K = tracks(C, n)
     ctx = pkg.MocapContext(C)
@@ -45,6 +82,8 @@ def case(C, n, reps):
         "calibrate_init_ransac": lambda: ctx.calibrate_init(obs, mask, method="ransac"),
         "ransac_stage": lambda: ctx.fundamental_ransac(obs, mask),
         "calculate_camera_poses_robust": lambda: pkg.calculate_camera_poses(image_points, session=session, robust=True),
+        "calculate_camera_poses_robust_screened": lambda: pkg.calculate_camera_poses(image_points, session=session, robust=True,
+                                                                                      reject_px=REJECT_PX),
         "cv2_fm_ransac_cpu": lambda: cv2_pairs(obs, mask),
     }
     ms = {k: [] for k in variants}
@@ -56,8 +95,9 @@ def case(C, n, reps):
             t0 = time.perf_counter()
             fn()
             ms[k].append((time.perf_counter() - t0) * 1e3)
-    return {"cameras": C, "points": n, "reps": reps,
-            **{k: {"median_ms": float(np.median(v)), "min_ms": float(np.min(v)), "max_ms": float(np.max(v))} for k, v in ms.items()}}
+    return {"cameras": C, "points": n, "reps": reps, "reject_px": REJECT_PX,
+            **{k: {"median_ms": float(np.median(v)), "min_ms": float(np.min(v)), "max_ms": float(np.max(v))} for k, v in ms.items()},
+            **({"screen": screen_kernel_ms(obs, mask, K)} if C == 16 else {})}
 
 
 if __name__ == "__main__":
