@@ -188,6 +188,30 @@ MOCAP_API int mocap_locate_objects_dev(mocap_ctx* ctx, const double* obj, const 
                              int n_frame_sets, int max_objects, double* objects, int32_t* drone_index,
                              int32_t* n_objects);
 
+/* Drone tracking -- replaces KalmanFilter.predict_location (KalmanFilter.py:50-100, with its LowPassFilter.py
+ * filters) for n_frame_sets frame-sets at once; each frame-set is one predict_location call at its timestamp.  A
+ * tracker holds device-resident state for num_objects (1 .. 8) drones on one context and enqueues on the context's
+ * stream; create it after the context's stream is set as wanted, destroy it before the context.
+ *   mocap_tracker_reset(tr, prev_time): the reference's reset() with prev_time = its time.time() - 20: the next
+ *   present step of every drone re-initialises at its first candidate and prev_positions returns to zero; the
+ *   covariance and the low-pass histories are kept.  Applied by the next mocap_track_objects_dev call.
+ *   mocap_track_objects_dev: objects / drone_index / n_objects / max_objects are mocap_locate_objects_dev's outputs,
+ *   timestamps double [n_frame_sets] in seconds (a frame-set with no objects only advances time).  Outputs per
+ *   frame-set and drone: pos float [n_frame_sets][num_objects][3], vel float [..][3] (low-pass filtered), heading
+ *   double [..] (low-pass filtered), present uint8 [..] (1 where the reference returns a record for the drone),
+ *   chosen int32 [..] (the object row the drone was associated with, -1 if absent); pos / vel / heading are 0 where
+ *   present is 0.  DEVICE pointers, two launches, never synchronises (the first batch larger than the tracker's
+ *   buffers waits for the stream while they grow).  A NULL pointer, max_objects < 1 or n_frame_sets < 1 returns
+ *   MOCAP_EINVAL before any launch. */
+typedef struct mocap_tracker mocap_tracker;
+MOCAP_API int  mocap_tracker_create(mocap_ctx* ctx, int num_objects, mocap_tracker** out);
+MOCAP_API void mocap_tracker_destroy(mocap_tracker* tr);
+MOCAP_API int  mocap_tracker_reset(mocap_tracker* tr, double prev_time);
+MOCAP_API int  mocap_track_objects_dev(mocap_tracker* tr, const double* objects, const int32_t* drone_index,
+                                       const int32_t* n_objects, int max_objects, const double* timestamps,
+                                       int n_frame_sets, float* pos, float* vel, double* heading, uint8_t* present,
+                                       int32_t* chosen);
+
 /* S3 -- replaces triangulate_points (helpers.py:330-336) and
  * calculate_reprojection_errors (helpers.py:203-211) on explicit correspondences.
  * obs double [n_points][n_cam][2], mask uint8 [n_points][n_cam] (0 = [None, None]).

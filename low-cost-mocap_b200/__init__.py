@@ -20,4 +20,6 @@ from .api import (  # noqa: F401
     locate_objects,
     calculate_camera_poses,
     install_into,
+    KalmanFilter,
+    Tracker,
 )

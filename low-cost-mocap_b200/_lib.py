@@ -84,6 +84,10 @@ SYMBOLS = {
     "mocap_pipeline_tracks_dev": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P]),
     "mocap_screen_observations_dev": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, _P, C.c_double, _P, _P]),
     "mocap_screen_observations_host": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, _P, C.c_double, _P, _P]),
+    "mocap_tracker_create": (C.c_int, [_P, C.c_int, C.POINTER(_P)]),
+    "mocap_tracker_destroy": (None, [_P]),
+    "mocap_tracker_reset": (C.c_int, [_P, C.c_double]),
+    "mocap_track_objects_dev": (C.c_int, [_P, _P, _P, _P, C.c_int, _P, C.c_int, _P, _P, _P, _P, _P]),
     "mocap_ba_residuals_host": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, _P, _P, C.POINTER(C.c_int)]),
     "mocap_host_alloc": (C.c_int, [C.POINTER(_P), C.c_uint64]),
     "mocap_host_free": (None, [_P]),

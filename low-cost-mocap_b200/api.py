@@ -17,6 +17,7 @@ from __future__ import annotations
 
 import ctypes as C
 import threading
+import time
 
 import numpy as np
 
@@ -416,6 +417,11 @@ class MocapContext:
         self._check(self.lib.mocap_locate_objects_dev(self.h, _ptr(obj), _ptr(err), _ptr(n), B, max_objects, _ptr(out), _ptr(di), _ptr(cnt)))
         return {"objects": out, "drone_index": di, "n": cnt}
 
+    def tracker(self, num_objects=2):
+        """A batched drone tracker on this context (:class:`Tracker`): the reference's KalmanFilter.predict_location
+        for whole batches of located frame-sets, state kept on the device between batches."""
+        return Tracker(self, num_objects)
+
     # -- explicit correspondences (host arrays) -------------------------------------------
     def triangulate(self, obs, mask, want_err=True):
         """obs float64 [F, C, 2], mask uint8 [F, C] -> (X [F,3], err [F] or None, valid [F])."""
@@ -521,6 +527,60 @@ class MocapContext:
         ms, n = C.c_double(0), C.c_int(0)
         self._check(self.lib.mocap_detect_kernel_ms(self.h, 1 if reset else 0, C.byref(ms), C.byref(n)))
         return ms.value, n.value
+
+
+class Tracker:
+    """Device-resident state of the reference's ``KalmanFilter(num_objects)`` (mocap_tracker_*): one Kalman filter and
+    three low-pass filters per drone.  Every frame-set of a batch counts as one ``predict_location`` call at its
+    timestamp; frame-sets without objects only advance time.  Enqueues on torch's current stream, never synchronises.
+    Close it (or drop it) before its context."""
+
+    def __init__(self, ctx, num_objects=2):
+        self.ctx, self.num_objects = ctx, int(num_objects)
+        h = C.c_void_p()
+        ctx._check(ctx.lib.mocap_tracker_create(ctx.h, self.num_objects, C.byref(h)))
+        self.h = h
+
+    def close(self):
+        if getattr(self, "h", None) and getattr(self.ctx, "h", None):
+            self.ctx.lib.mocap_tracker_destroy(self.h)
+        self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def reset(self, prev_time):
+        """The reference's ``reset()`` with its clock reading: ``prev_time`` = that reading - 20 s.  Takes effect at the
+        next batch: every drone re-initialises at its next present step; covariances and low-pass histories stay."""
+        self.ctx._check(self.ctx.lib.mocap_tracker_reset(self.h, float(prev_time)))
+
+    def track_dev(self, located, timestamps, out=None):
+        """located: the dict ``MocapContext.locate_objects`` returns (objects f64 [B, M, 5], drone_index int32 [B, M],
+        n int32 [B]); timestamps: f64 cuda tensor [B] (seconds, one per frame-set).  Returns dict of cuda tensors, per
+        frame-set and drone: pos f32 [B, D, 3], vel f32 [B, D, 3] and heading f64 [B, D] (low-pass filtered), present
+        uint8 [B, D] and chosen int32 [B, D] (the object row, -1 if absent); pos / vel / heading are 0 where present
+        is 0.  Two launches."""
+        torch = _torch()
+        obj, di, n = located["objects"], located["drone_index"], located["n"]
+        B, M = obj.shape[0], obj.shape[1]
+        D = self.num_objects
+        dev = obj.device
+        if tuple(timestamps.shape) != (B,) or timestamps.dtype != torch.float64:
+            raise ValueError("timestamps must be a float64 tensor with one entry per frame-set")
+        if out is None:
+            out = {"pos": torch.empty((B, D, 3), dtype=torch.float32, device=dev),
+                   "vel": torch.empty((B, D, 3), dtype=torch.float32, device=dev),
+                   "heading": torch.empty((B, D), dtype=torch.float64, device=dev),
+                   "present": torch.empty((B, D), dtype=torch.uint8, device=dev),
+                   "chosen": torch.empty((B, D), dtype=torch.int32, device=dev)}
+        self.ctx.use_current_stream()
+        self.ctx._check(self.ctx.lib.mocap_track_objects_dev(self.h, _ptr(obj.contiguous()), _ptr(di.contiguous()), _ptr(n.contiguous()),
+                                                             M, _ptr(timestamps.contiguous()), B, _ptr(out["pos"]), _ptr(out["vel"]),
+                                                             _ptr(out["heading"]), _ptr(out["present"]), _ptr(out["chosen"])))
+        return out
 
 
 # =================================================================================================
@@ -709,6 +769,46 @@ def locate_objects(object_points, errors, session=None):
             for i in range(k)]
 
 
+class KalmanFilter:
+    """Mirror of the reference's ``KalmanFilter`` (KalmanFilter.py): ``predict_location(objects)`` takes the list
+    ``locate_objects`` returns and gives the list of ``{"pos": f32[3], "vel": f32[3], "heading": float64,
+    "droneIndex": d}`` for the drones among the objects; ``reset()`` as the reference's.  Each call is a batch of one
+    on a device tracker (``MocapContext.tracker``) and reads ``clock`` once (the reference reads ``time.time()`` twice
+    per call)."""
+
+    def __init__(self, num_objects, session=None, clock=time.time):
+        self.num_objects = int(num_objects)
+        self.session = session or MocapSession.default()
+        self.clock = clock
+        s = self.session
+        with s._lock:
+            self._ctx = s.ctx(len(s.intrinsics), **MIRROR_LIMITS)
+            self._tracker = self._ctx.tracker(self.num_objects)
+
+    def predict_location(self, objects):
+        torch = _torch()
+        now = float(self.clock())
+        M = max(1, len(objects))
+        obj = np.zeros((1, M, 5), dtype=np.float64)
+        di = np.full((1, M), -1, dtype=np.int32)
+        for i, o in enumerate(objects):
+            obj[0, i, :3] = np.asarray(o["pos"], dtype=np.float64).reshape(3)
+            obj[0, i, 3] = o["heading"]
+            d = o["droneIndex"]
+            di[0, i] = d if 0 <= d < self.num_objects else -1
+        dev = self._ctx.torch_device
+        with self.session._lock:
+            located = {"objects": torch.from_numpy(obj).to(dev), "drone_index": torch.from_numpy(di).to(dev),
+                       "n": torch.tensor([len(objects)], dtype=torch.int32, device=dev)}
+            r = self._tracker.track_dev(located, torch.tensor([now], dtype=torch.float64, device=dev))
+            r = {k: v[0].cpu().numpy() for k, v in r.items()}
+        return [{"pos": r["pos"][d].copy(), "vel": r["vel"][d].copy(), "heading": np.float64(r["heading"][d]), "droneIndex": d}
+                for d in range(self.num_objects) if r["present"][d]]
+
+    def reset(self):
+        self._tracker.reset(float(self.clock()) - 20)
+
+
 def bundle_adjustment(image_points, camera_poses, socketio, session=None):
     """Mirror of helpers.py:244-290: returns the list of ``{"R": ndarray 3x3, "t": ndarray (3,)}``.
     ``socketio.emit("camera-pose", ...)`` fires once with the result (the reference emits on
@@ -764,14 +864,18 @@ PATCHED_NAMES = ("triangulate_point", "triangulate_points", "calculate_reproject
                  "bundle_adjustment", "locate_objects")
 
 
-def install_into(helpers_module, *also, session=None):
+def install_into(helpers_module, *also, session=None, tracker=False):
     """Point a loaded reference ``helpers`` module at the CUDA path (INTEGRATION.md).
 
     ``also``: modules that imported the hot-path names BY VALUE -- the reference's ``index.py`` does
     (``from helpers import ... bundle_adjustment, triangulate_points, calculate_reprojection_errors``,
     index.py:1), so ``calculate_camera_pose`` (index.py:254,272,274,275) would keep the CPU functions.
     Every name of PATCHED_NAMES such a module holds is re-bound as well:
-    ``install_into(helpers, sys.modules[__name__])`` from inside index.py."""
+    ``install_into(helpers, sys.modules[__name__])`` from inside index.py.
+
+    ``tracker=True`` also re-binds ``KalmanFilter`` (in helpers and in every module of ``also`` that holds it) to
+    :class:`KalmanFilter` on this session, which ``start_trangulating_points`` (helpers.py:175) looks up at call
+    time; the default leaves the reference's CPU filter in place."""
     cams = helpers_module.Cameras.instance()
     s = session or MocapSession.install([np.asarray(p["intrinsic_matrix"], dtype=np.float64) for p in cams.camera_params])
     # helpers.Cameras is a Singleton WRAPPER object (Singleton.py:17-37); _camera_read looks _find_dot up on the
@@ -794,4 +898,15 @@ def install_into(helpers_module, *also, session=None):
         for mod in also:
             if hasattr(mod, name):
                 setattr(mod, name, fn)
+    if tracker:
+        class _KalmanFilter(KalmanFilter):
+            __mocap_b200__ = True
+
+            def __init__(self, num_objects, session=None, clock=time.time):
+                super().__init__(num_objects, session or s, clock)
+        _KalmanFilter.__name__ = _KalmanFilter.__qualname__ = "KalmanFilter"
+        setattr(helpers_module, "KalmanFilter", _KalmanFilter)
+        for mod in also:
+            if hasattr(mod, "KalmanFilter"):
+                setattr(mod, "KalmanFilter", _KalmanFilter)
     return s
