@@ -267,6 +267,53 @@ MOCAP_API int  mocap_calibrate_init_ransac_host(mocap_ctx* ctx, const double* ob
 MOCAP_API int  mocap_fundamental_ransac_host(mocap_ctx* ctx, const double* obs, const uint8_t* mask, int n_points,
                                    const mocap_ransac_options* opt, double* F, uint8_t* inliers);
 
+/* Pose-graph cold start: every camera placed from every overlapping pair instead of the chain of adjacent pairs.
+ * It computes what the reference's calculate-camera-pose handler computes (index.py:229-270) -- the camera poses in
+ * camera 0's frame with |t_1| = 1, from 2D tracks and the intrinsics -- and departs from it deliberately:
+ *   - every pair (a < b) with at least min_common common observations is used, not only (c, c+1): one bad pair no
+ *     longer breaks the cameras after it;
+ *   - each pair's F comes from RANSAC (as mocap_calibrate_init_ransac_host, pair p of the pair table drawing its
+ *     samples from (seed, p)), re-fitted by 8-point rounds on its Sampson inliers;
+ *   - E = K_b^T F K_a with each pair's own intrinsics (the reference uses those of cameras 0 and 1, index.py:247), and
+ *     the four motions are judged in the pair's own frame, P_a = K_a [I|0], P_b = K_b [R|t], counting the inliers in
+ *     front of both cameras (the reference triangulates with camera a's accumulated pose on one side and the relative
+ *     candidate on the other, index.py:253-262, which can pick a twisted motion);
+ *   - a pair is dropped with fewer than min_inliers points in front or a median triangulation angle below
+ *     min_angle_deg; rotations by weighted chordal averaging with Cauchy re-weighting, pairs off by more than
+ *     rot_outlier_deg dropped;
+ *   - translations from the bearing constraints of every track with the rotations known (the reference chains
+ *     t_{c+1} = t_c + R_c t_rel with unit baselines, index.py:264-265), irls_rounds rounds of Cauchy weights at 4 px;
+ *     a view enters if it is an inlier of at least 2 used pairs (1 where its camera has one used pair).
+ * HOST pointers.  ropt / gopt NULL = defaults.  R [n_cam][9], t [n_cam][3] out.  pairs (capacity n_cam(n_cam-1)/2,
+ * may be NULL) receives one record per pair of the pair table, *n_pairs (may be NULL) their number.  support uint8
+ * [n_points][n_cam] (may be NULL): 1 where the view's final weight is >= 0.5 on a track that keeps at least 2 such
+ * views -- a first bundle-adjustment mask.  Bad options, too few common observations to link every camera to camera 0
+ * or more than 16 cameras return MOCAP_EINVAL before any launch; if the pairs that pass the checks no longer link every
+ * camera, MOCAP_EINVAL names the cameras.  Device scratch grows with pairs x hypotheses x 27 doubles (53 MB at 120
+ * pairs x 2048, 425 MB at 16384); MOCAP_ECUDA if it cannot be allocated.  Two calls with the same inputs give the same
+ * bits. */
+typedef struct mocap_graph_options {
+    int    min_common;        /* 30: common observations for a pair to enter the table, >= 8 */
+    int    min_inliers;       /* 30: inliers in front of both cameras for a pair to be used   */
+    double min_angle_deg;     /* 2.0: median triangulation angle for a pair to be used        */
+    double rot_outlier_deg;   /* 5.0: rotation residual above which a pair is dropped         */
+    int    irls_rounds;       /* 4: translation solves, 1 .. 64                               */
+} mocap_graph_options;
+typedef struct mocap_graph_pair {
+    int    a, b;              /* cameras, a < b                                               */
+    int    common;            /* common observations                                          */
+    int    inliers;           /* Sampson inliers of the re-fitted F                           */
+    int    candidate;         /* chosen motion 0..3 of E, -1 if none                           */
+    int    in_front;          /* inliers in front of both cameras under it                    */
+    double median_angle_deg;  /* median triangulation angle of those                          */
+    double rot_residual_deg;  /* angle between R_b R_a^T and the pair's R_ab (NaN: no motion) */
+    int    used;              /* 1 if the pair placed the rotations and chose the views       */
+} mocap_graph_pair;
+MOCAP_API void mocap_graph_default_options(mocap_graph_options* opt);
+MOCAP_API int  mocap_calibrate_graph_host(mocap_ctx* ctx, const double* obs, const uint8_t* mask, int n_points,
+                                const mocap_ransac_options* ropt, const mocap_graph_options* gopt, double* R, double* t,
+                                mocap_graph_pair* pairs, int* n_pairs, uint8_t* support);
+
 /* S4 -- replaces bundle_adjustment (helpers.py:244-290): robust (Cauchy) trust-region
  * least squares over the poses of cameras 1..C-1 (rotation vector + translation;
  * camera 0 pinned at (I,0); the reference's focal parameters are dead, helpers.py:267-270),

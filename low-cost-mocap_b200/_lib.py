@@ -41,6 +41,16 @@ class RansacOptions(C.Structure):
     _fields_ = [("threshold_px", C.c_double), ("hypotheses", C.c_int), ("seed", C.c_uint64)]
 
 
+class GraphOptions(C.Structure):
+    _fields_ = [("min_common", C.c_int), ("min_inliers", C.c_int), ("min_angle_deg", C.c_double), ("rot_outlier_deg", C.c_double),
+                ("irls_rounds", C.c_int)]
+
+
+class GraphPair(C.Structure):
+    _fields_ = [("a", C.c_int), ("b", C.c_int), ("common", C.c_int), ("inliers", C.c_int), ("candidate", C.c_int),
+                ("in_front", C.c_int), ("median_angle_deg", C.c_double), ("rot_residual_deg", C.c_double), ("used", C.c_int)]
+
+
 class BAProblem(C.Structure):
     _fields_ = [("obs", C.c_void_p), ("mask", C.c_void_p), ("n_points_max", C.c_int), ("n_points", C.c_void_p),
                 ("R", C.c_void_p), ("t", C.c_void_p), ("report", C.c_void_p)]
@@ -75,6 +85,9 @@ SYMBOLS = {
     "mocap_ransac_default_options": (None, [C.POINTER(RansacOptions)]),
     "mocap_calibrate_init_ransac_host": (C.c_int, [_P, _P, _P, C.c_int, C.POINTER(RansacOptions), _P, _P, _P, _P, _P]),
     "mocap_fundamental_ransac_host": (C.c_int, [_P, _P, _P, C.c_int, C.POINTER(RansacOptions), _P, _P]),
+    "mocap_graph_default_options": (None, [C.POINTER(GraphOptions)]),
+    "mocap_calibrate_graph_host": (C.c_int, [_P, _P, _P, C.c_int, C.POINTER(RansacOptions), C.POINTER(GraphOptions), _P, _P,
+                                             _P, C.POINTER(C.c_int), _P]),
     "mocap_ba_default_options": (None, [C.POINTER(BAOptions)]),
     "mocap_bundle_adjust_host": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, C.POINTER(BAOptions), C.POINTER(BAReport)]),
     "mocap_bundle_adjust_dev": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, _P, C.POINTER(BAOptions), _P]),

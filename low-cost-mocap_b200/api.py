@@ -22,7 +22,7 @@ import time
 import numpy as np
 
 from . import _lib
-from ._lib import MocapError, Config, BAOptions, BAProblem, BAReport, RansacOptions, check
+from ._lib import MocapError, Config, BAOptions, BAProblem, BAReport, RansacOptions, GraphOptions, GraphPair, check
 
 THRESHOLD = 51   # cv.threshold(grey, 255*0.2, 255, THRESH_BINARY) on uint8 == pix > 51 (helpers.py:146)
 
@@ -450,16 +450,29 @@ class MocapContext:
         opt.threshold_px, opt.hypotheses, opt.seed = float(threshold), int(hypotheses), int(seed)
         return opt
 
-    def calibrate_init(self, obs, mask, F_given=None, method="8point", threshold=1.0, hypotheses=2048, seed=0):
+    def calibrate_init(self, obs, mask, F_given=None, method="8point", threshold=1.0, hypotheses=2048, seed=0, **graph_options):
         """Chain of relative poses from 2D tracks (index.py:229-270).  Returns (poses, F_used [C-1,3,3], votes [C-1,4]).
 
         ``method="8point"``: each pair's F is a normalised 8-point fit to all common observations, re-fitted on its
         1 px Sampson inliers (or ``F_given``).  ``method="ransac"``: the fit starts from the inliers of a RANSAC model
         (``hypotheses`` 7-point samples per pair from ``seed``, inliers within ``threshold`` px), which mismatched
-        points do not pull; the return then also holds the per-pair inlier masks, uint8 [F, C-1]."""
+        points do not pull; the return then also holds the per-pair inlier masks, uint8 [F, C-1].
+
+        ``method="graph"``: every camera placed from every overlapping pair (mocap_calibrate_graph_host, DESIGN section
+        1 (f) #4): RANSAC F for all pairs with at least ``min_common`` common observations, the motion chosen in each
+        pair's own frame, rotation averaging and the translations of all tracks at once.  ``graph_options`` are the
+        fields of ``mocap_graph_options`` (min_common, min_inliers, min_angle_deg, rot_outlier_deg, irls_rounds).
+        Returns (poses, pairs, support): pairs a list of dicts (a, b, common, inliers, candidate, in_front,
+        median_angle_deg, rot_residual_deg, used), support uint8 [F, C] -- a first bundle-adjustment mask."""
         obs = np.ascontiguousarray(obs, dtype=np.float64)
         mask = np.ascontiguousarray(mask, dtype=np.uint8)
         Cn = self.n_cam
+        if method == "graph":
+            if F_given is not None:
+                raise ValueError("calibrate_init: F_given and method='graph' exclude each other")
+            return self._calibrate_graph(obs, mask, threshold, hypotheses, seed, graph_options)
+        if graph_options:
+            raise ValueError(f"calibrate_init: {sorted(graph_options)} apply to method='graph' only")
         R = np.empty((Cn, 3, 3)); t = np.empty((Cn, 3))
         Fu = np.empty((Cn - 1, 3, 3)); votes = np.empty((Cn - 1, 4), dtype=np.int32)
         if method == "ransac":
@@ -471,11 +484,30 @@ class MocapContext:
                                                                   _np_ptr(R), _np_ptr(t), _np_ptr(Fu), _np_ptr(votes), _np_ptr(inl)))
             return [{"R": R[i].copy(), "t": t[i].copy()} for i in range(Cn)], Fu, votes, inl
         if method != "8point":
-            raise ValueError(f"calibrate_init: unknown method {method!r} (expected '8point' or 'ransac')")
+            raise ValueError(f"calibrate_init: unknown method {method!r} (expected '8point', 'ransac' or 'graph')")
         Fg = None if F_given is None else np.ascontiguousarray(np.asarray(F_given, dtype=np.float64).reshape(Cn - 1, 3, 3))
         self._check(self.lib.mocap_calibrate_init_host(self.h, _np_ptr(obs), _np_ptr(mask), obs.shape[0], _np_ptr(Fg),
                                                        _np_ptr(R), _np_ptr(t), _np_ptr(Fu), _np_ptr(votes)))
         return [{"R": R[i].copy(), "t": t[i].copy()} for i in range(Cn)], Fu, votes
+
+    def _calibrate_graph(self, obs, mask, threshold, hypotheses, seed, graph_options):
+        Cn = self.n_cam
+        gopt = GraphOptions()
+        self.lib.mocap_graph_default_options(C.byref(gopt))
+        for k, v in graph_options.items():
+            if k not in dict(GraphOptions._fields_):
+                raise ValueError(f"calibrate_init: unknown graph option {k!r} (expected one of "
+                                 f"{', '.join(f for f, _ in GraphOptions._fields_)})")
+            setattr(gopt, k, v)
+        opt = self._ransac_options(threshold, hypotheses, seed)
+        R = np.empty((Cn, 3, 3)); t = np.empty((Cn, 3))
+        pairs = (GraphPair * max(1, Cn * (Cn - 1) // 2))()
+        n_pairs = C.c_int(0)
+        support = np.zeros(mask.shape, dtype=np.uint8)
+        self._check(self.lib.mocap_calibrate_graph_host(self.h, _np_ptr(obs), _np_ptr(mask), obs.shape[0], C.byref(opt), C.byref(gopt),
+                                                        _np_ptr(R), _np_ptr(t), pairs, C.byref(n_pairs), _np_ptr(support)))
+        rep = [{f: getattr(pairs[i], f) for f, _ in GraphPair._fields_} for i in range(n_pairs.value)]
+        return [{"R": R[i].copy(), "t": t[i].copy()} for i in range(Cn)], rep, support
 
     def fundamental_ransac(self, obs, mask, threshold=1.0, hypotheses=2048, seed=0):
         """The RANSAC stage of ``calibrate_init(method="ransac")`` alone: per adjacent pair the winning 7-point model
@@ -822,7 +854,7 @@ def bundle_adjustment(image_points, camera_poses, socketio, session=None):
     return out
 
 
-def calculate_camera_poses(image_points, socketio=None, session=None, robust=False, reject_px=None, rounds=2):
+def calculate_camera_poses(image_points, socketio=None, session=None, robust=False, reject_px=None, rounds=2, init="chain"):
     """The computation of the reference's ``calculate-camera-pose`` handler (index.py:229-277): cold-start
     chain of relative poses, then bundle adjustment.  ``image_points`` is the (F, C, 2) list the UI sends
     (``data["cameraPoints"]``) with ``None`` for missing views.  ``robust=True`` starts the chain from RANSAC
@@ -830,7 +862,11 @@ def calculate_camera_poses(image_points, socketio=None, session=None, robust=Fal
     reflection recorded as a camera's first point -- do not pull.  ``reject_px`` (None: every view enters the
     adjustment, as in the reference) screens views that disagree with their track by more than that many pixels out
     of the adjustment, ``rounds`` times (``MocapContext.bundle_adjust_screened``; INTEGRATION.md recommends a value).
-    Returns the list of {"R", "t"}."""
+    ``init="graph"`` starts from the pose graph of every overlapping camera pair instead of the chain
+    (``MocapContext.calibrate_init(method="graph")``; RANSAC is implied, ``robust`` is ignored); with ``reject_px`` the
+    first solve then sees the views the graph's translation step supports.  Returns the list of {"R", "t"}."""
+    if init not in ("chain", "graph"):
+        raise ValueError(f"calculate_camera_poses: unknown init {init!r} (expected 'chain' or 'graph')")
     s = session or MocapSession.default()
     obs, mask = _split_observations(image_points)
     n_cam = obs.shape[1]
@@ -838,14 +874,17 @@ def calculate_camera_poses(image_points, socketio=None, session=None, robust=Fal
         ctx = s.ctx(n_cam)
         ident = [{"R": np.eye(3), "t": np.zeros(3)} for _ in range(n_cam)]
         ctx.set_cameras(s.intrinsics[:n_cam], ident)
-        init = ctx.calibrate_init(obs, mask, method="ransac" if robust else "8point")
+        graph = init == "graph"
+        init = ctx.calibrate_init(obs, mask, method="graph" if graph else ("ransac" if robust else "8point"))
         start = init[0]
         ctx.set_cameras(s.intrinsics[:n_cam], start)
         if reject_px is None:
             out, _ = ctx.bundle_adjust(obs, mask, start)
         else:
             first = None
-            if robust:
+            if graph:
+                first = init[2]
+            elif robust:
                 # the first solve sees the views that are RANSAC inliers with a neighbouring camera; the screens that
                 # follow start from every view again
                 inl = init[3].astype(bool)

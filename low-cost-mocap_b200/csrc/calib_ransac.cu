@@ -91,20 +91,72 @@ k_ransac_mask(const float4* __restrict__ pts, const int* __restrict__ off, int H
 
 static size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
 
+int ransac_check_options(mocap_ctx* ctx, const mocap_ransac_options* opt, mocap_ransac_options* o, const char* who) {
+    mocap_ransac_default_options(o);
+    if (opt) *o = *opt;
+    if (!(o->threshold_px > 0) || !isfinite(o->threshold_px) || o->hypotheses < 1 || o->hypotheses > RS_MAX_HYP)
+        return mocap_fail(ctx, MOCAP_EINVAL, "%s: threshold_px must be positive and finite and hypotheses in 1..%d (got %g, %d)", who,
+                          RS_MAX_HYP, o->threshold_px, o->hypotheses);
+    return MOCAP_OK;
+}
+
+size_t ransac_scratch_bytes(int P, size_t total, int H) {
+    return align256(total * sizeof(float4)) + align256((P + 1) * sizeof(int)) + align256((size_t)P * H * 27 * sizeof(double)) +
+           align256((size_t)P * H * sizeof(int)) + align256(P * sizeof(unsigned long long)) + align256(P * 9 * sizeof(double)) +
+           align256(total);
+}
+
+int ransac_run(mocap_ctx* ctx, const float4* h_pts, const int* h_off, int P, const mocap_ransac_options& o, double* F_best,
+               uint8_t* inl, unsigned long long* keys) {
+    const int H = o.hypotheses;
+    const double thr2 = o.threshold_px * o.threshold_px;
+    const size_t total = (size_t)h_off[P];
+    CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));
+    const size_t b_pts = align256(total * sizeof(float4)), b_off = align256((P + 1) * sizeof(int));
+    const size_t b_models = align256((size_t)P * H * 27 * sizeof(double)), b_n = align256((size_t)P * H * sizeof(int));
+    const size_t b_best = align256(P * sizeof(unsigned long long)), b_F = align256(P * 9 * sizeof(double));
+    int st = ensure_scratch(ctx, ransac_scratch_bytes(P, total, H));
+    if (st) return st;
+    unsigned char* b = static_cast<unsigned char*>(ctx->d_scratch);
+    float4* d_pts = reinterpret_cast<float4*>(b); b += b_pts;
+    int* d_off = reinterpret_cast<int*>(b); b += b_off;
+    double* d_models = reinterpret_cast<double*>(b); b += b_models;
+    int* d_n = reinterpret_cast<int*>(b); b += b_n;
+    unsigned long long* d_best = reinterpret_cast<unsigned long long*>(b); b += b_best;
+    double* d_F = reinterpret_cast<double*>(b); b += b_F;
+    uint8_t* d_inl = b;
+    cudaStream_t s = ctx->stream;
+    CUDA_TRY(ctx, cudaMemcpyAsync(d_pts, h_pts, total * sizeof(float4), cudaMemcpyHostToDevice, s));
+    CUDA_TRY(ctx, cudaMemcpyAsync(d_off, h_off, (P + 1) * sizeof(int), cudaMemcpyHostToDevice, s));
+    CUDA_TRY(ctx, cudaMemsetAsync(d_best, 0, P * sizeof(unsigned long long), s));
+    k_ransac_hypotheses<<<dim3((H + RS_HYP_THREADS - 1) / RS_HYP_THREADS, P), RS_HYP_THREADS, 0, s>>>(
+        d_pts, d_off, H, (unsigned long long)o.seed, d_models, d_n);
+    CUDA_TRY(ctx, cudaGetLastError());
+    k_ransac_score<<<dim3((H + RS_SCORE_WARPS - 1) / RS_SCORE_WARPS, P), RS_SCORE_WARPS * 32, 0, s>>>(d_pts, d_off, H, thr2, d_models,
+                                                                                                      d_n, d_best);
+    CUDA_TRY(ctx, cudaGetLastError());
+    const int mmax = [&] { int x = 0; for (int c = 0; c < P; ++c) x = h_off[c + 1] - h_off[c] > x ? h_off[c + 1] - h_off[c] : x; return x; }();
+    k_ransac_mask<<<dim3((mmax + 255) / 256 < 32 ? (mmax + 255) / 256 : 32, P), 256, 0, s>>>(d_pts, d_off, H, thr2, d_models, d_best,
+                                                                                            d_inl, d_F);
+    CUDA_TRY(ctx, cudaGetLastError());
+    ctx->launches += 3;
+    CUDA_TRY(ctx, cudaMemcpyAsync(keys, d_best, P * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(ctx, cudaMemcpyAsync(F_best, d_F, P * 9 * sizeof(double), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(ctx, cudaMemcpyAsync(inl, d_inl, total, cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(ctx, cudaStreamSynchronize(s));
+    return MOCAP_OK;
+}
+
 // RANSAC over every adjacent pair: F_best [C-1][9] and, per pair, the inlier mask over its common observations in
-// frame order (inl, pair after pair; off [C] gives each pair's start).  Validates everything before any launch.
+// frame order (inl, pair after pair; off [C] gives each pair's start).  Pair p is cameras (p, p+1).  Validates
+// everything before any launch.
 static int ransac_pairs(mocap_ctx* ctx, const double* obs, const uint8_t* mask, int n_points, const mocap_ransac_options* opt,
                  double* F_best, std::vector<uint8_t>& inl, std::vector<int>& off, const char* who) {
     const int C = ctx->cfg.n_cam, P = C - 1;
     if (!obs || !mask || n_points < 8 || C < 2) return mocap_fail(ctx, MOCAP_EINVAL, "%s: bad argument", who);
     mocap_ransac_options o;
-    mocap_ransac_default_options(&o);
-    if (opt) o = *opt;
-    if (!(o.threshold_px > 0) || !isfinite(o.threshold_px) || o.hypotheses < 1 || o.hypotheses > RS_MAX_HYP)
-        return mocap_fail(ctx, MOCAP_EINVAL, "%s: threshold_px must be positive and finite and hypotheses in 1..%d (got %g, %d)", who,
-                          RS_MAX_HYP, o.threshold_px, o.hypotheses);
-    const int H = o.hypotheses;
-    const double thr2 = o.threshold_px * o.threshold_px;
+    int st = ransac_check_options(ctx, opt, &o, who);
+    if (st) return st;
     std::vector<float4> pts;
     off.assign(C, 0);
     for (int c = 0; c < P; ++c) {
@@ -118,42 +170,10 @@ static int ransac_pairs(mocap_ctx* ctx, const double* obs, const uint8_t* mask, 
         if (m < 8) return mocap_fail(ctx, MOCAP_EINVAL, "%s: cameras %d and %d share only %d observations", who, c, c + 1, m);
     }
     off[P] = (int)pts.size();
-    const size_t total = pts.size();
-    CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));
-    const size_t b_pts = align256(total * sizeof(float4)), b_off = align256((P + 1) * sizeof(int));
-    const size_t b_models = align256((size_t)P * H * 27 * sizeof(double)), b_n = align256((size_t)P * H * sizeof(int));
-    const size_t b_best = align256(P * sizeof(unsigned long long)), b_F = align256(P * 9 * sizeof(double));
-    int st = ensure_scratch(ctx, b_pts + b_off + b_models + b_n + b_best + b_F + align256(total));
-    if (st) return st;
-    unsigned char* b = static_cast<unsigned char*>(ctx->d_scratch);
-    float4* d_pts = reinterpret_cast<float4*>(b); b += b_pts;
-    int* d_off = reinterpret_cast<int*>(b); b += b_off;
-    double* d_models = reinterpret_cast<double*>(b); b += b_models;
-    int* d_n = reinterpret_cast<int*>(b); b += b_n;
-    unsigned long long* d_best = reinterpret_cast<unsigned long long*>(b); b += b_best;
-    double* d_F = reinterpret_cast<double*>(b); b += b_F;
-    uint8_t* d_inl = b;
-    cudaStream_t s = ctx->stream;
-    CUDA_TRY(ctx, cudaMemcpyAsync(d_pts, pts.data(), total * sizeof(float4), cudaMemcpyHostToDevice, s));
-    CUDA_TRY(ctx, cudaMemcpyAsync(d_off, off.data(), (P + 1) * sizeof(int), cudaMemcpyHostToDevice, s));
-    CUDA_TRY(ctx, cudaMemsetAsync(d_best, 0, P * sizeof(unsigned long long), s));
-    k_ransac_hypotheses<<<dim3((H + RS_HYP_THREADS - 1) / RS_HYP_THREADS, P), RS_HYP_THREADS, 0, s>>>(
-        d_pts, d_off, H, (unsigned long long)o.seed, d_models, d_n);
-    CUDA_TRY(ctx, cudaGetLastError());
-    k_ransac_score<<<dim3((H + RS_SCORE_WARPS - 1) / RS_SCORE_WARPS, P), RS_SCORE_WARPS * 32, 0, s>>>(d_pts, d_off, H, thr2, d_models,
-                                                                                                      d_n, d_best);
-    CUDA_TRY(ctx, cudaGetLastError());
-    const int mmax = [&] { int x = 0; for (int c = 0; c < P; ++c) x = off[c + 1] - off[c] > x ? off[c + 1] - off[c] : x; return x; }();
-    k_ransac_mask<<<dim3((mmax + 255) / 256 < 32 ? (mmax + 255) / 256 : 32, P), 256, 0, s>>>(d_pts, d_off, H, thr2, d_models, d_best,
-                                                                                            d_inl, d_F);
-    CUDA_TRY(ctx, cudaGetLastError());
-    ctx->launches += 3;
     std::vector<unsigned long long> keys(P);
-    inl.resize(total);
-    CUDA_TRY(ctx, cudaMemcpyAsync(keys.data(), d_best, P * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
-    CUDA_TRY(ctx, cudaMemcpyAsync(F_best, d_F, P * 9 * sizeof(double), cudaMemcpyDeviceToHost, s));
-    CUDA_TRY(ctx, cudaMemcpyAsync(inl.data(), d_inl, total, cudaMemcpyDeviceToHost, s));
-    CUDA_TRY(ctx, cudaStreamSynchronize(s));
+    inl.resize(pts.size());
+    st = ransac_run(ctx, pts.data(), off.data(), P, o, F_best, inl.data(), keys.data());
+    if (st) return st;
     for (int c = 0; c < P; ++c)
         if (!keys[c]) return mocap_fail(ctx, MOCAP_EINVAL, "%s: no 7-point sample of cameras %d and %d gave a model", who, c, c + 1);
     return MOCAP_OK;

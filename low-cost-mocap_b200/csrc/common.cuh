@@ -121,3 +121,12 @@ int timing_flush(mocap_ctx* ctx);
 // observations) and re-fitted on its Sampson inliers at thr2, E, the cheirality vote and the chain
 int calibrate_chain(mocap_ctx* ctx, const double* obs, const uint8_t* mask, int n_points, const double* F_given,
                     const uint8_t* init_inl, double thr2, double* R, double* t, double* F_used, int* votes, uint8_t* inl_out);
+// RANSAC fundamental matrices over a list of camera pairs (calib_ransac.cu).  ransac_check_options fills o (opt NULL =
+// defaults) or fails with MOCAP_EINVAL.  ransac_run: h_pts holds every pair's common observations {x_a, y_a, x_b, y_b}
+// (float32), pair p at [h_off[p], h_off[p+1]); pair p's samples are drawn from the hash of (seed, p, ...).  Out: F_best
+// [P][9], inl over h_pts, keys [P] (0: no sample of that pair gave a model).  Three launches, one synchronisation.
+// Scratch: ransac_scratch_bytes, dominated by P * hypotheses * 27 doubles of models.
+int ransac_check_options(mocap_ctx* ctx, const mocap_ransac_options* opt, mocap_ransac_options* o, const char* who);
+size_t ransac_scratch_bytes(int P, size_t total, int H);
+int ransac_run(mocap_ctx* ctx, const float4* h_pts, const int* h_off, int P, const mocap_ransac_options& o, double* F_best,
+               uint8_t* inl, unsigned long long* keys);

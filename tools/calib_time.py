@@ -4,7 +4,8 @@ alone (fundamental_ransac: three kernels for all pairs), and calculate_camera_po
 cameras x 6400 points (16 x 6400 is BASELINE config 5: 64 markers x 100 frames), 10 % of each camera's observations
 mismatched; calculate_camera_poses(robust=True, reject_px=REJECT_PX) beside it, and at 16 cameras the screen kernel
 alone (CUDA events over many launches, each with its stats reset) and one bundle-adjustment solve of the screened
-tracks.  Beside them the CPU time of cv2.findFundamentalMat(FM_RANSAC, 1 px, 0.99999) over the same pairs, the
+tracks.  The pose-graph initialiser (calibrate_init(method="graph"), calculate_camera_poses(init="graph", reject_px))
+beside the chain, and at 16 cameras its device time per kernel (torch.profiler over one call).  Beside them the CPU time of cv2.findFundamentalMat(FM_RANSAC, 1 px, 0.99999) over the same pairs, the
 reference handler's estimator.  Every entry point synchronises before it returns, so a host clock around each call
 measures it; the variants are alternated and medians reported.  Prints one JSON document (GPU name and power limit
 included); --out also writes it to a file."""
@@ -72,6 +73,29 @@ def screen_kernel_ms(obs, mask, K, launches=200, solves=10):
             "ba_solve_after_screen_ms_median": float(np.median(solve))}
 
 
+def graph_kernel_ms(obs, mask, K, calls=3):
+    """Device time per kernel of calibrate_init(method="graph"), summed over its launches and averaged over `calls`
+    calls (torch.profiler, CUDA activity), with the number of launches per call."""
+    from torch.profiler import ProfilerActivity, profile
+    C = obs.shape[1]
+    ctx = pkg.MocapContext(C)
+    ctx.set_cameras([K] * C, [{"R": np.eye(3), "t": np.zeros(3)}] * C)
+    ctx.calibrate_init(obs, mask, method="graph")
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(calls):
+            ctx.calibrate_init(obs, mask, method="graph")
+        torch.cuda.synchronize()
+    out = {}
+    for ev in prof.key_averages():
+        if ev.key.startswith("k_"):
+            dev_us = getattr(ev, "device_time_total", None)
+            if dev_us is None:
+                dev_us = ev.cuda_time_total
+            out[ev.key] = {"ms_per_call": dev_us / 1e3 / calls, "launches_per_call": ev.count / calls}
+    return out
+
+
 def case(C, n, reps):
     obs, mask, image_points, K = tracks(C, n)
     ctx = pkg.MocapContext(C)
@@ -84,6 +108,9 @@ def case(C, n, reps):
         "calculate_camera_poses_robust": lambda: pkg.calculate_camera_poses(image_points, session=session, robust=True),
         "calculate_camera_poses_robust_screened": lambda: pkg.calculate_camera_poses(image_points, session=session, robust=True,
                                                                                       reject_px=REJECT_PX),
+        "calibrate_init_graph": lambda: ctx.calibrate_init(obs, mask, method="graph"),
+        "calculate_camera_poses_graph_screened": lambda: pkg.calculate_camera_poses(image_points, session=session, init="graph",
+                                                                                     reject_px=REJECT_PX),
         "cv2_fm_ransac_cpu": lambda: cv2_pairs(obs, mask),
     }
     ms = {k: [] for k in variants}
@@ -97,7 +124,7 @@ def case(C, n, reps):
             ms[k].append((time.perf_counter() - t0) * 1e3)
     return {"cameras": C, "points": n, "reps": reps, "reject_px": REJECT_PX,
             **{k: {"median_ms": float(np.median(v)), "min_ms": float(np.min(v)), "max_ms": float(np.max(v))} for k, v in ms.items()},
-            **({"screen": screen_kernel_ms(obs, mask, K)} if C == 16 else {})}
+            **({"screen": screen_kernel_ms(obs, mask, K), "graph_kernels": graph_kernel_ms(obs, mask, K)} if C == 16 else {})}
 
 
 if __name__ == "__main__":
