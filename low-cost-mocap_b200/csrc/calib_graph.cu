@@ -287,6 +287,7 @@ static bool fit_from_normal(const double* up, const double T[6], double F[9]) {
     mat3mul(M2t, Fr, tmp); mat3mul(tmp, M1, F);
     double nf = 0; for (int i = 0; i < 9; ++i) nf += F[i] * F[i];
     nf = sqrt(nf); if (nf > 0) for (int i = 0; i < 9; ++i) F[i] /= nf;
+    fix_sign(F);
     return true;
 }
 

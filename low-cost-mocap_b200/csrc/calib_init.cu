@@ -150,6 +150,7 @@ static int pair_motion(mocap_ctx* ctx, const double* d_p1, const double* d_p2, u
             mat3mul(M2t, Fr, tmp); mat3mul(tmp, M1, F);
             double nf = 0; for (int i = 0; i < 9; ++i) nf += F[i] * F[i];
             nf = sqrt(nf); if (nf > 0) for (int i = 0; i < 9; ++i) F[i] /= nf;
+            fix_sign(F);
             if (round == 2) break;
             // Sampson inliers at thr2 (1 px: the reference's RANSAC threshold, index.py:246)
             int* d_cnt = reinterpret_cast<int*>(d_work + 64);

@@ -67,6 +67,16 @@ inline void mat3mul(const double A[9], const double B[9], double C[9]) {
     for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) { double x = 0; for (int k = 0; k < 3; ++k) x += A[3 * i + k] * B[3 * k + j]; C[3 * i + j] = x; }
 }
 
+// Sign of a fitted F (9 entries): the entry of largest magnitude made positive (the first of equal magnitudes).  The
+// smallest eigenvector's sign is otherwise whatever the eigen solver's rounding makes it: two summation orders of the
+// same normal matrix (the device's and a host model's, or two runs under floating-point atomics) can give opposite
+// signs, and with them the four motions of E in another order.
+inline void fix_sign(double F[9]) {
+    int k = 0;
+    for (int i = 1; i < 9; ++i) if (fabs(F[i]) > fabs(F[k])) k = i;
+    if (F[k] < 0) for (int i = 0; i < 9; ++i) F[i] = -F[i];
+}
+
 // libmv MotionFromEssential (cv.sfm.motionFromEssential, index.py:248): Rs = [UWV^T, UWV^T, UW^TV^T, UW^TV^T],
 // ts = [u3, -u3, u3, -u3], after flipping the last column of U / last row of V^T when their determinant is negative
 inline void motion_from_essential(const double E[9], double Rs[4][9], double ts[4][3]) {

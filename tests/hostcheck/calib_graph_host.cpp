@@ -50,6 +50,56 @@ double hc_cheirality(const double* Ka, const double* Kb, const double* R, const 
     return a;
 }
 
+// Every correspondence of a pair under one candidate, as k_pair_cheirality sees it: pts [m][4] float32 {xa, ya, xb, yb},
+// inl [m].  front [m] and ang [m] (-1 where not an inlier or not in front) out; margin [m] out: the smaller of |X_z| and
+// |(R X + t)_z| over |X|, how far the front decision lies from its threshold (inf where not an inlier).
+void hc_cheirality_pair(const double* Ka, const double* Kb, const double* R, const double* t, const float* pts, const uint8_t* inl, int m,
+                        uint8_t* front, double* ang, double* margin) {
+    const double I3[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1}, z3[3] = {0, 0, 0};
+    double Pa[12], Pb[12];
+    cg_make_P(Ka, I3, z3, Pa);
+    cg_make_P(Kb, R, t, Pb);
+    for (int i = 0; i < m; ++i) {
+        front[i] = 0; ang[i] = -1.0; margin[i] = INFINITY;
+        if (!inl[i]) continue;
+        const double xa = pts[4 * i], ya = pts[4 * i + 1], xb = pts[4 * i + 2], yb = pts[4 * i + 3];
+        bool f;
+        const double a = cg_cheirality_point(Pa, Pb, R, t, xa, ya, xb, yb, f);
+        if (f) { front[i] = 1; ang[i] = a; }
+        Sym4 B;
+        sym4_zero(B);
+        dlt_add_view(B, Pa, xa, ya);
+        dlt_add_view(B, Pb, xb, yb);
+        double X[3];
+        dlt_solve(B, X);
+        const double zb = R[6] * X[0] + R[7] * X[1] + R[8] * X[2] + t[2];
+        margin[i] = fmin(fabs(X[2]), fabs(zb)) / sqrt(X[0] * X[0] + X[1] * X[1] + X[2] * X[2]);
+    }
+}
+
+// F from the 45-entry upper triangle of a normal matrix in normalised coordinates and T = {s1, tx1, ty1, s2, tx2, ty2}:
+// the arithmetic of fit_from_normal (calib_graph.cu) and of pair_motion (calib_init.cu) -- smallest eigenvector by
+// trf::sym_eig, rank 2 by svd3, de-normalised, unit norm, with the product's sign.  Returns 0 if the eigen problem fails.
+int hc_fit_from_normal(const double* up, const double* T, double* F) {
+    using namespace calib_pose;
+    std::vector<double> A(81), lam;
+    int k = 0;
+    for (int r = 0; r < 9; ++r) for (int c = r; c < 9; ++c) { A[9 * r + c] = up[k]; A[9 * c + r] = up[k]; ++k; }
+    if (!trf::sym_eig(9, A, lam)) return 0;
+    int best = 0;
+    for (int i = 1; i < 9; ++i) if (lam[i] < lam[best]) best = i;
+    double Fn[9], U[9], sv[3], V[9], Fr[9], tmp[9];
+    for (int i = 0; i < 9; ++i) Fn[i] = A[9 * i + best];
+    svd3(Fn, U, sv, V);
+    for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) Fr[3 * i + j] = U[3 * i] * sv[0] * V[3 * j] + U[3 * i + 1] * sv[1] * V[3 * j + 1];
+    const double M1[9] = {T[0], 0, T[1], 0, T[0], T[2], 0, 0, 1}, M2t[9] = {T[3], 0, 0, 0, T[3], 0, T[4], T[5], 1};
+    mat3mul(M2t, Fr, tmp); mat3mul(tmp, M1, F);
+    double nf = 0; for (int i = 0; i < 9; ++i) nf += F[i] * F[i];
+    nf = sqrt(nf); if (nf > 0) for (int i = 0; i < 9; ++i) F[i] /= nf;
+    fix_sign(F);
+    return 1;
+}
+
 void hc_motion_from_essential(const double* E, double* Rs /*[4][9]*/, double* ts /*[4][3]*/) {
     double R4[4][9], t4[4][3];
     calib_pose::motion_from_essential(E, R4, t4);

@@ -53,4 +53,24 @@ int hc_ransac_select(const float* pts, int m, int p, int H, uint64_t seed, doubl
     for (int i = 0; i < m; ++i) mask[i] = rs_is_inlier(F_out, q[i].x, q[i].y, q[i].z, q[i].w, thr2) ? 1 : 0;
     return 1;
 }
+
+// Every model of hc_ransac_select's scan: n_models [H], counts [H][3] (-1 past a hypothesis' models), F [H][3][9]
+void hc_ransac_models(const float* pts, int m, int p, int H, uint64_t seed, double thr, int* n_models, int* counts, double* F) {
+    const HP4* q = reinterpret_cast<const HP4*>(pts);
+    const double thr2 = thr * thr;
+    for (int h = 0; h < H; ++h) {
+        double Fh[3][9];
+        const int n = rs_hypothesis(q, m, seed, p, h, Fh);
+        n_models[h] = n;
+        for (int k = 0; k < 3; ++k) {
+            int c = -1;
+            if (k < n) {
+                c = 0;
+                for (int i = 0; i < m; ++i) c += rs_is_inlier(Fh[k], q[i].x, q[i].y, q[i].z, q[i].w, thr2) ? 1 : 0;
+                memcpy(F + 27 * (size_t)h + 9 * k, Fh[k], sizeof(Fh[k]));
+            }
+            counts[3 * h + k] = c;
+        }
+    }
+}
 }

@@ -11,6 +11,7 @@ import numpy as np
 import pytest
 from scipy import stats
 
+from tests.calib_util import eight_point_refit
 from tests.util import ROOT
 
 synth = importlib.import_module("low-cost-mocap_b200.synth")
@@ -55,38 +56,6 @@ def contaminated_pair(seed, frac, n=200):
     bad[rng.choice(n, int(round(frac * n)), replace=False)] = True
     x2[bad] = np.floor(rng.uniform([0, 0], [synth.WIDTH, synth.HEIGHT], size=(bad.sum(), 2)))
     return x1, x2, np.asarray(poses[1]["R"]), K, bad
-
-
-def eight_point_refit(x1, x2, inl0, thr=1.0):
-    """numpy restatement of calib_init.cu's pair_motion estimator started from a given fit set: normalised 8-point,
-    rank 2, then re-fits on the Sampson inliers, three fits in all."""
-    n = len(x1)
-    inl = inl0.copy() if inl0.sum() >= 8 else np.ones(n, dtype=bool)
-    for r in range(3):
-        def T(h):
-            c = h[inl].mean(0)
-            s = np.sqrt(2) / np.linalg.norm(h[inl] - c, axis=1).mean()
-            return np.array([[s, 0, -s * c[0]], [0, s, -s * c[1]], [0, 0, 1]])
-        T1, T2 = T(x1), T(x2)
-        a = np.c_[x1, np.ones(n)] @ T1.T
-        b = np.c_[x2, np.ones(n)] @ T2.T
-        A = np.einsum("ni,nj->nij", b, a).reshape(n, 9)[inl]
-        Fn = np.linalg.eigh(A.T @ A)[1][:, 0].reshape(3, 3)
-        U, s, Vt = np.linalg.svd(Fn)
-        F = T2.T @ (U @ np.diag([s[0], s[1], 0]) @ Vt) @ T1
-        F /= np.linalg.norm(F)
-        if r == 2:
-            break
-        h1, h2 = np.c_[x1, np.ones(n)], np.c_[x2, np.ones(n)]
-        l, m = h1 @ F.T, h2 @ F
-        e = (h2 * l).sum(1)
-        new = e * e / (l[:, 0] ** 2 + l[:, 1] ** 2 + m[:, 0] ** 2 + m[:, 1] ** 2) <= thr * thr
-        if new.sum() < 8:
-            new[:] = True
-        if new.all() and r > 0:
-            break
-        inl = new
-    return F
 
 
 def rotation_error_deg(F, K, R_true):
