@@ -34,7 +34,10 @@
  *               layout Cameras._find_dot receives, helpers.py:143)
  *   blob_xy     int32  [n_images][max_blobs][2]   (x, y) = int(m10/m00), int(m01/m00)
  *   blob_n      int32  [n_images]                 n_images = n_frame_sets * n_cam
- *   blob_mom    int64  [n_images][max_blobs][4]   {2*m00, 6*m10, 6*m01, pixel count}
+ *   blob_mom    int64  [n_images][max_blobs][4]   {2*m00, 6*m10, 6*m01, pixel count}; the pixel count of a
+ *                                                 blob is its 8-connected area, that of a hole contour the size
+ *                                                 of the region the hole encloses: its 4-connected component of
+ *                                                 the complement of the blob around it, nested blobs included
  *   img_flags   int32  [n_images]                 MOCAP_F_* bits
  *   obj         double [n_frame_sets][max_roots][3]
  *   err         double [n_frame_sets][max_roots]  mean squared reprojection error, px^2
@@ -69,7 +72,9 @@ extern "C" {
                                  cv.moments treat them (helpers.py:147-158): one more contour -- one more point -- per hole, the
                                  outer contour's moments over the FILLED blob, cv2's hierarchy order.  The bit is left only
                                  when that slow path could not run: a holed blob wider or taller than 62 pixels, or more
-                                 than 64 holes in the image; the image then carries one centre per blob from its set pixels. */
+                                 than 64 holes in the image; the image then carries, for every blob of it, holed or not,
+                                 one centre and the moments of the polygon through its own set pixels, in descending
+                                 raster order of the blob's first pixel, as an image without holes does. */
 
 #if defined(__GNUC__)
 #define MOCAP_API __attribute__((visibility("default")))

@@ -309,7 +309,14 @@ __device__ __noinline__ void blob_holes_cta(BlobSmem sm, int n, unsigned n_runs,
     if (tid == 0) {
         int count = 0;
         if (hs.unsupported) {
-            // as the fast path: one centre per blob from its own (by now partly filled) moments, reverse raster order
+            // as the fast path: one centre per blob from its set pixels, reverse raster order.  The blobs handled before
+            // the limit was met (and the one at which the hole cap was reached, in part) had their holes' moments added
+            // above; every such hole is recorded, so taking them out again restores the set-pixel sums exactly.
+            for (int j = 0; j < hs.nholes; ++j) {
+                const unsigned b = hs.hblob[j];
+                acc_add<WIDE>(sm.acc, 4 * b, -hs.hA2[j]); acc_add<WIDE>(sm.acc, 4 * b + 1, -hs.hSX6[j]);
+                acc_add<WIDE>(sm.acc, 4 * b + 2, -hs.hSY6[j]);
+            }
             for (int k = (int)nb - 1; k >= 0; --k) {
                 const unsigned long long A2 = acc_get<WIDE>(sm.acc, 4 * k);
                 if (!A2) continue;

@@ -15,8 +15,9 @@
 //
 // This is the slow path: it runs in the full-size (one CTA per image) reduction only -- the one-warp-per-image fast
 // path hands images whose Euler numbers show a hole to the worklist -- on a 64 x 64 bitmap window per holed blob.
-// A holed blob wider or taller than 62 pixels, or more than HOLE_CAP holes in one image, is left as the fast path
-// computes it and the image keeps MOCAP_F_HOLES; otherwise the bit is cleared: the result is the reference's.
+// A holed blob wider or taller than 62 pixels, or more than HOLE_CAP holes in one image, makes the whole image leave as
+// the fast path computes it (one centre per blob from its set pixels: the hole moments already added are taken out
+// again) and the image keeps MOCAP_F_HOLES; otherwise the bit is cleared: the result is the reference's.
 #pragma once
 #include "common.cuh"
 

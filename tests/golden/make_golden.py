@@ -120,8 +120,9 @@ def irregular_blob_case(name, n_frames, seed):
 def ring_blob_case(name, n_frames, seed):
     """S1 on blobs WITH holes (rings, frames, porous patches, nested blobs) next to solid ones: what the real
     _find_dot returns (one extra point per hole contour, hole-filled outer moments) and, per frame, whether cv2's
-    contour hierarchy contains a hole.  The CUDA path does not reproduce RETR_TREE on such blobs; it must raise
-    MOCAP_F_HOLES exactly on these frames and agree exactly on the others."""
+    contour hierarchy contains a hole.  The CUDA path reproduces RETR_TREE on such blobs (csrc/blob_holes.cuh) and must
+    agree exactly on every frame within the limits of that path; beyond them (a holed blob wider or taller than 62 px,
+    more than 64 holes in one image) it keeps MOCAP_F_HOLES."""
     import cv2
     helpers, cams = load_reference(1)
     rng = np.random.default_rng(seed)

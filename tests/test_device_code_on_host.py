@@ -115,7 +115,7 @@ def test_capacity_paths_of_the_blob_code(blob_emu):
             d[y - 1:y + 2, x - 1:x + 2] = 255
             y = int(np.clip(y + rng.integers(-2, 3), 2, 477)); x = int(np.clip(x + rng.integers(-2, 3), 2, 637))
     import cv2
-    d = cv2.morphologyEx(d, cv2.MORPH_CLOSE, np.ones((5, 5), np.uint8))   # solid blobs (no holes): the S1 contract
+    d = cv2.morphologyEx(d, cv2.MORPH_CLOSE, np.ones((5, 5), np.uint8))   # solid blobs: this test is about capacities
     filled = d.copy()
     contours, _ = cv2.findContours(d, cv2.RETR_EXTERNAL, cv2.CHAIN_APPROX_NONE)
     cv2.drawContours(filled, contours, -1, 255, thickness=cv2.FILLED)
@@ -417,7 +417,7 @@ def test_blob_device_code_fuzz_vs_cv2(blob_emu):
         cv2.drawContours(img, contours, -1, 255, thickness=cv2.FILLED)
         _, hier = cv2.findContours(img, cv2.RETR_CCOMP, cv2.CHAIN_APPROX_NONE)
         if hier is not None and (hier[0][:, 3] >= 0).any():
-            continue                                          # a hole survived: outside the S1 contract (DESIGN.md section 7)
+            continue                                          # a hole survived: holed blobs are the RETR_TREE test's
         grey = (img > 0).astype(np.uint8) * int(rng.integers(60, 256))
         ref = [q for q in port.find_dot(np.repeat(grey[:, :, None], 3, axis=2)) if q[0] is not None]
         for force_cta in (0, 1):
@@ -596,20 +596,17 @@ def test_blob_device_code_reproduces_retr_tree_on_blobs_with_holes(blob_emu):
     a hole to the full-size reduction, which runs the RETR_TREE slow path (csrc/blob_holes.cuh): the emitted points
     -- count, values and order -- equal cv2's on random images with rings, frames, porous patches, blobs inside holes,
     rings inside rings, holes touching diagonally, 1-px walls, blobs across the 16-px segment boundaries and at the
-    image border; no flag is left.  A holed blob too large for the slow path's window keeps MOCAP_F_HOLES."""
+    image border; no flag is left.  The moments are cv2's integers for every contour, hole contours included, and the
+    pixel count of a hole is the size of the region it encloses.  A holed blob too large for the slow path's window
+    keeps MOCAP_F_HOLES."""
     import cv2
+    from tests.util import retr_tree_blobs
     rng = np.random.default_rng(31)
     H, W = 96, 128
 
     def reference(img):
-        contours, hier = cv2.findContours((img > 51).astype(np.uint8), cv2.RETR_TREE, cv2.CHAIN_APPROX_SIMPLE)
-        out = []
-        for cnt in contours:
-            m = cv2.moments(cnt)
-            if m["m00"] != 0:
-                out.append([int(m["m10"] / m["m00"]), int(m["m01"] / m["m00"])])
-        has_hole = hier is not None and any(h[3] >= 0 for h in hier[0])
-        return out, has_hole
+        items, _, _, holes = retr_tree_blobs(img > 51)
+        return items, holes > 0
     seen = {True: 0, False: 0}
     for trial in range(50):
         img = np.zeros((H, W), np.uint8)
@@ -639,7 +636,8 @@ def test_blob_device_code_reproduces_retr_tree_on_blobs_with_holes(blob_emu):
         seen[has_hole] += 1
         for force_cta in (0, 1):
             d = blob_emu(img, force_cta=force_cta, seed=trial)
-            assert d["flags"] == 0 and d["xy"].tolist() == ref, (trial, force_cta, d["flags"])
+            got = [tuple(int(v) for v in d["mom"][i]) + tuple(int(v) for v in d["xy"][i]) for i in range(d["n"])]
+            assert d["flags"] == 0 and got == ref, (trial, force_cta, d["flags"])
             if has_hole:
                 assert d["path"] == 2                    # the slow path lives in the full-size reduction
     assert seen[True] >= 15                           # (solid-only images are what every other blob test covers)
@@ -647,6 +645,42 @@ def test_blob_device_code_reproduces_retr_tree_on_blobs_with_holes(blob_emu):
     cv2.circle(big, (64, 48), 40, 255, 2)                # an 84-px ring: wider than the 62-px window
     d = blob_emu(big)
     assert d["flags"] == 32 and d["n"] == 1
+
+
+def test_blob_device_code_flagged_image_reports_set_pixel_moments(blob_emu):
+    """An image the RETR_TREE slow path cannot take (more than 64 holes, a holed blob wider than 62 px) keeps
+    MOCAP_F_HOLES and reports one centre per blob from its SET pixels, in reverse raster order -- also for the holed
+    blobs the slow path had already filled before it met the limit, and for the blob at which it met the hole cap.
+    One hole fewer, the same image is reproduced as cv2 sees it."""
+    from tests.util import porous_patch, retr_tree_blobs, set_pixel_blobs
+    H, W = 128, 160
+
+    def two_patches(n_second):
+        img = np.zeros((H, W), np.uint8)
+        img[10:27, 10:31] = porous_patch(40)
+        img[60:77, 90:111] = porous_patch(n_second)            # across the 16-px segment border at x = 96
+        return img
+    for n_second, flagged in ((40, True), (25, True), (24, False)):
+        img = two_patches(n_second)
+        ref = set_pixel_blobs(img) if flagged else retr_tree_blobs(img)[0]
+        assert len(ref) == (2 if flagged else 2 + 40 + n_second)
+        for force_cta in (0, 1):
+            d = blob_emu(img, max_blobs=128, force_cta=force_cta)
+            got = [tuple(int(v) for v in d["mom"][i]) + tuple(int(v) for v in d["xy"][i]) for i in range(d["n"])]
+            assert d["flags"] == (32 if flagged else 0) and got == ref, (n_second, force_cta, got, ref[:2])
+    assert [r[0] for r in set_pixel_blobs(two_patches(40))] == [480, 480]
+    # a 16-px frame beside a 71-px frame: the small one fits the window and was filled before the big one was met
+    import cv2
+    img = np.zeros((H, W), np.uint8)
+    cv2.rectangle(img, (10, 10), (25, 25), 255, 1)
+    img[11:14, 11:13] = 255                                     # lopsided: the filled and set-pixel centres differ
+    cv2.rectangle(img, (40, 50), (110, 89), 255, 1)
+    ref = set_pixel_blobs(img)
+    assert ref[1][:3] != retr_tree_blobs(img[:30, :30])[0][0][:3]
+    for force_cta in (0, 1):
+        d = blob_emu(img, force_cta=force_cta)
+        got = [tuple(int(v) for v in d["mom"][i]) + tuple(int(v) for v in d["xy"][i]) for i in range(d["n"])]
+        assert d["flags"] == 32 and got == ref, (force_cta, got, ref)
 
 
 def test_single_pass_kernel_on_host_three_channel_layout(fused_emu):

@@ -614,8 +614,8 @@ def test_preprocess_bit_exact_vs_cv2_chain(torch):
         assert np.array_equal(m1, r1) and np.array_equal(m2, r2)
     rng = np.random.default_rng(4)
     raw = rng.integers(0, 256, size=(3, C, 240, 320, 3), dtype=np.uint8)
-    # marker-like frames: dark clutter + bright Gaussian spots (stay solid through blur + sharpen;
-    # hard-edged discs turn into rings, i.e. blobs with holes, which are outside the S1 contract)
+    # marker-like frames: dark clutter + bright Gaussian spots (stay solid through blur + sharpen; hard-edged discs
+    # turn into rings, i.e. blobs with holes: tests/test_gpu_holes.py runs those through the raw-frame chain)
     yy, xx = np.mgrid[:240, :320]
     for b in range(1, 3):
         raw[b] = rng.integers(0, 30, size=(C, 240, 320, 3), dtype=np.uint8)
@@ -819,7 +819,7 @@ def _random_solid_frame(rng, H, W, n_shapes):
             cv2.fillPoly(img, [pts], val)
         else:
             img[cy:cy + int(rng.integers(1, 6)), cx:cx + int(rng.integers(1, 20))] = val
-    binary = (img > 51).astype(np.uint8)                 # fill holes: the S1 contract is solid blobs
+    binary = (img > 51).astype(np.uint8)                 # fill holes: this fuzz is of solid blobs (holed ones: test_gpu_holes.py)
     ff = binary.copy()
     cv2.floodFill(ff, np.zeros((H + 2, W + 2), np.uint8), (0, 0), 1)
     if binary[0, 0]:

@@ -51,6 +51,96 @@ def as3(img):
     return np.repeat(img[:, :, None], 3, axis=2).copy()
 
 
+# ------------------------------------------------------------------------- S1 references for blobs with holes
+def porous_patch(n_holes, h=17, w=21):
+    """An h x w block with n_holes one-pixel holes on the odd rows and columns, filled from the top: each hole opens
+    the four cells around it, so the set-pixel and the filled polygon differ in area and in centre."""
+    m = np.full((h, w), 255, np.uint8)
+    spots = [(y, x) for y in range(1, h - 1, 2) for x in range(1, w - 1, 2)]
+    assert n_holes <= len(spots)
+    for y, x in spots[:n_holes]:
+        m[y, x] = 0
+    return m
+
+
+def _centre(A2, SX6, SY6):
+    """int(m10/m00) of the device's emission, in the same float64 operations."""
+    m00 = float(A2) * 0.5
+    return [int(float(SX6) * 0.16666666666666666 / m00), int(float(SY6) * 0.16666666666666666 / m00)]
+
+
+def retr_tree_blobs(binary):
+    """What cv.findContours(RETR_TREE, CHAIN_APPROX_SIMPLE) + cv.moments make of a binary image, in cv2's order, contours
+    of zero area dropped (helpers.py:147-158): a list of (A2, SX6, SY6, npix, x, y) -- the integers 2*m00, 6*m10, 6*m01;
+    npix is a blob's pixel count (connectedComponentsWithStats, 8-connectivity) or, for a hole, the size of the region
+    it encloses: its 4-connected component of the complement of the blob around it, nested blobs included.
+    Returns (items, number of kept hole contours, the holed blobs' largest bounding-box side, number of holes)."""
+    import cv2
+    from scipy import ndimage
+    binary = (np.asarray(binary) != 0).astype(np.uint8)
+    contours, hier = cv2.findContours(binary, cv2.RETR_TREE, cv2.CHAIN_APPROX_SIMPLE)
+    if not contours:
+        return [], 0, 0, 0
+    _, lab, stats, _ = cv2.connectedComponentsWithStats(binary, connectivity=8)
+    parent = hier[0][:, 3]
+    items, kept_holes, side, holes, fills = [], 0, 0, 0, {}
+    for i, cnt in enumerate(contours):
+        depth, p = 0, parent[i]
+        while p >= 0:
+            depth, p = depth + 1, parent[p]
+        x0, y0 = (int(v) for v in cnt[0, 0])
+        blob = lab[y0, x0]
+        if depth % 2:                                  # a hole border runs through pixels of the blob around the hole
+            if blob not in fills:                      # the complement's 4-components inside the blob's bounding box
+                bx, by, bw, bh = (int(v) for v in stats[blob, :4])
+                fills[blob] = (bx, by, lab[by:by + bh, bx:bx + bw] != blob)
+                fills[blob] += (ndimage.label(fills[blob][2])[0],)
+                side = max(side, bw, bh)
+            bx, by, other, region = fills[blob]
+            inside = np.zeros(other.shape, np.uint8)
+            cv2.drawContours(inside, [cnt], 0, 1, thickness=cv2.FILLED, offset=(-bx, -by))
+            ids = np.unique(region[(inside != 0) & other])
+            assert len(ids) == 1, ids                  # exactly one enclosed region per hole contour
+            npix = int((region == ids[0]).sum())
+            holes += 1
+        else:
+            npix = int(stats[blob, cv2.CC_STAT_AREA])
+        m = cv2.moments(cnt)
+        if m["m00"] != 0:
+            items.append((round(m["m00"] * 2), round(m["m10"] * 6), round(m["m01"] * 6), npix,
+                          int(m["m10"] / m["m00"]), int(m["m01"] / m["m00"])))
+            kept_holes += depth % 2
+    return items, kept_holes, side, holes
+
+
+def set_pixel_blobs(binary):
+    """One item (A2, SX6, SY6, npix, x, y) per 8-connected blob from the polygon through its own set pixels' centres --
+    the 2x2-cell sums of DESIGN.md section 5, holes left open -- in descending raster order of the blob's first pixel,
+    blobs of zero area dropped: what S1 reports for an image it flags with MOCAP_F_HOLES."""
+    import cv2
+    b = (np.asarray(binary) != 0)
+    n, lab, stats, _ = cv2.connectedComponentsWithStats(b.astype(np.uint8), connectivity=8)
+    tl, tr, bl, br = (c.astype(np.int64) for c in (b[:-1, :-1], b[:-1, 1:], b[1:, :-1], b[1:, 1:]))
+    cnt = tl + tr + bl + br
+    y, x = np.mgrid[:b.shape[0] - 1, :b.shape[1] - 1].astype(np.int64)
+    full, tri = cnt == 4, cnt == 3
+    a2 = 2 * full + tri
+    sx6 = np.where(full, 6 * x + 3, 0) + np.where(tri, tl * x + tr * (x + 1) + bl * x + br * (x + 1), 0)
+    sy6 = np.where(full, 6 * y + 3, 0) + np.where(tri, (tl + tr) * y + (bl + br) * (y + 1), 0)
+    cell_lab = np.maximum(np.maximum(lab[:-1, :-1], lab[:-1, 1:]), np.maximum(lab[1:, :-1], lab[1:, 1:]))   # one blob per cell
+    sums = np.zeros((n, 3), np.int64)
+    for k, v in enumerate((a2, sx6, sy6)):
+        np.add.at(sums[:, k], cell_lab.ravel(), v.ravel())
+    labels, first = np.unique(lab.ravel(), return_index=True)
+    out = []
+    for k in labels[np.argsort(-first)]:
+        if k == 0 or sums[k, 0] == 0:
+            continue
+        A2, SX6, SY6 = (int(v) for v in sums[k])
+        out.append((A2, SX6, SY6, int(stats[k, cv2.CC_STAT_AREA])) + tuple(_centre(A2, SX6, SY6)))
+    return out
+
+
 # ------------------------------------------------------------- DLT at near-degenerate geometry (S3 null vector)
 def _yaw(a):
     c, s = np.cos(a), np.sin(a)
