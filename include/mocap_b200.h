@@ -188,7 +188,9 @@ MOCAP_API int mocap_get_undistort_map(mocap_ctx* ctx, int cam, int16_t* m1, uint
  * records.  Input is the matcher's output (obj/err/n_obj, with the world transform set if the caller
  * wants world coordinates as the reference does).  objects double [n_frame_sets][max_objects][5] =
  * {x, y, z, heading, error}; drone_index int32 [n_frame_sets][max_objects]; n_objects int32
- * [n_frame_sets].  DEVICE pointers. */
+ * [n_frame_sets].  A frame-set's first min(n_obj, max_roots) points are read (n_obj <= 0: none).  A frame-set can hold up
+ * to one object per point; objects beyond max_objects (>= 1) are dropped in scan order, n_objects is clamped to
+ * max_objects and record slots at or beyond n_objects are left unwritten.  DEVICE pointers. */
 MOCAP_API int mocap_locate_objects_dev(mocap_ctx* ctx, const double* obj, const double* err, const int32_t* n_obj,
                              int n_frame_sets, int max_objects, double* objects, int32_t* drone_index,
                              int32_t* n_objects);

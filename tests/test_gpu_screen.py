@@ -198,9 +198,12 @@ def test_clean_tracks_lose_no_view_and_meet_the_8point_bar(torch):
     assert aligned_error(ctx, obs, mask, pts, final, K) < 0.03
 
 
-def test_default_keeps_the_unscreened_path(torch):
+def test_default_keeps_the_unscreened_path(torch, monkeypatch):
     """reject_px=None is the adjustment of every view: the same poses as bundle_adjust from the same chain, and as
-    bundle_adjust_screened with rounds=0."""
+    bundle_adjust_screened with rounds=0 -- bit for bit.  calculate_camera_poses builds its own chain, which agrees with
+    another run's to rounding only (calibrate_init's re-fits sum with atomics); on these 20 % mismatched tracks the
+    adjustment carries that 1e-13 to several 1e-5 in the final poses, so the API's poses are compared with bundle_adjust
+    from the very chain it built, recorded as it goes by."""
     C = 8
     obs, mask, obs_obj, _, _, K, _ = contaminated_tracks(C, 200, 0.2, seed=31)
     ctx = _ctx(C, K)
@@ -209,12 +212,28 @@ def test_default_keeps_the_unscreened_path(torch):
     plain, _ = ctx.bundle_adjust(obs, mask, start)
     zero, _, kept = ctx.bundle_adjust_screened(obs, mask, start, REJECT_PX, rounds=0)
     assert np.array_equal(kept, mask)
-    via_api = pkg.calculate_camera_poses(obs_obj.tolist(), session=pkg.MocapSession([K] * C), robust=True)
     for a, b in zip(plain, zero):
         assert np.array_equal(a["R"], b["R"]) and np.array_equal(a["t"], b["t"])
-    # the chain inside agrees with `start` to rounding only (calibrate_init's re-fits sum with atomics)
+    session = pkg.MocapSession([K] * C)
+    inner, chains = session.ctx(C), []
+    real = inner.calibrate_init
+
+    def recording(*a, **kw):
+        chains.append(real(*a, **kw))
+        return chains[-1]
+    monkeypatch.setattr(inner, "calibrate_init", recording)
+    via_api = pkg.calculate_camera_poses(obs_obj.tolist(), session=session, robust=True)
+    assert len(chains) == 1
+    own_start = chains[0][0]
+    for a, b in zip(start, own_start):
+        assert np.abs(np.asarray(a["R"]) - b["R"]).max() < 1e-9 and np.abs(np.ravel(a["t"]) - np.ravel(b["t"])).max() < 1e-9
+    ctx.set_cameras([K] * C, own_start)
+    same, _ = ctx.bundle_adjust(obs, mask, own_start)
+    for a, b in zip(same, via_api):
+        assert np.array_equal(a["R"], b["R"]) and np.array_equal(a["t"], b["t"])
+    # and from the other chain the adjustment ends at the same rig, to what it makes of the chains' rounding
     for a, b in zip(plain, via_api):
-        assert np.abs(a["R"] - b["R"]).max() < 1e-4 and np.abs(a["t"] - b["t"]).max() < 1e-4
+        assert np.abs(a["R"] - b["R"]).max() < 1e-3 and np.abs(a["t"] - b["t"]).max() < 1e-3
 
 
 @pytest.mark.parametrize("rounds", [0, 1, 2, 3])
