@@ -71,10 +71,12 @@ extern "C" {
 #define MOCAP_F_HOLES    32   /* per image, not an overflow.  Blobs with holes are reproduced as cv.findContours(RETR_TREE) +
                                  cv.moments treat them (helpers.py:147-158): one more contour -- one more point -- per hole, the
                                  outer contour's moments over the FILLED blob, cv2's hierarchy order.  The bit is left only
-                                 when that slow path could not run: a holed blob wider or taller than 62 pixels, or more
-                                 than 64 holes in the image; the image then carries, for every blob of it, holed or not,
-                                 one centre and the moments of the polygon through its own set pixels, in descending
-                                 raster order of the blob's first pixel, as an image without holes does. */
+                                 when that slow path could not run.  By default: a holed blob wider or taller than 62
+                                 pixels, or more than 64 holes in the image.  With mocap_set_large_holes(ctx, 1): more
+                                 than 64 holes in the image only (a holed blob of any size is reproduced).  The image then
+                                 carries, for every blob of it, holed or not, one centre and the moments of the polygon
+                                 through its own set pixels, in descending raster order of the blob's first pixel, as an
+                                 image without holes does. */
 
 #if defined(__GNUC__)
 #define MOCAP_API __attribute__((visibility("default")))
@@ -130,6 +132,16 @@ MOCAP_API int mocap_set_world_transform(mocap_ctx* ctx, const double* M);
 MOCAP_API int mocap_detect_dev(mocap_ctx* ctx, const uint8_t* frames, int n_images, int channels,
                      int threshold, int32_t* blob_xy, int32_t* blob_n,
                      int64_t* blob_mom, int32_t* img_flags);
+
+/* Holed blobs wider or taller than 62 pixels in S1 (every entry point that runs S1).  cv.findContours(RETR_TREE) +
+ * cv.moments (helpers.py:147-158) give such a blob a contour per hole and fill its outer one, whatever its size; by
+ * default (off) S1 reproduces that for holed blobs up to 62 x 62 pixels only and flags an image with a larger one
+ * (MOCAP_F_HOLES).  on != 0 allocates a whole-image window for the slow path, four bitmaps of (height + 2) x
+ * ceil((width + 2) / 64) 64-bit words per SM (166 KB per SM at 640 x 480, 409 KB at 1024 x 768), and larger holed
+ * blobs are reproduced too: only more than 64 holes in one image leave the flag.  on == 0 frees it.  Results of images
+ * the default already reproduces do not change.  Synchronises the context's stream; MOCAP_ENOMEM when the allocation
+ * fails (the setting is then off). */
+MOCAP_API int mocap_set_large_holes(mocap_ctx* ctx, int on);
 
 /* S2+S3 -- replaces find_point_correspondance_and_object_points (helpers.py:339-421),
  * incl. the triangulate_points / calculate_reprojection_errors calls inside it

@@ -69,6 +69,7 @@ SYMBOLS = {
     "mocap_set_stream": (C.c_int, [_P, _P]),
     "mocap_set_cameras": (C.c_int, [_P, _P, _P, _P]),
     "mocap_set_world_transform": (C.c_int, [_P, _P]),
+    "mocap_set_large_holes": (C.c_int, [_P, C.c_int]),
     "mocap_detect_dev": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _P, _P, _P, _P]),
     "mocap_match_triangulate_dev": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, _P, _P, _P]),
     "mocap_pipeline_dev": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _P, _P, _P, _P]),

@@ -41,7 +41,7 @@ def raise_on_overflow(flags, what):
     if flags & F_HOLES:
         raise MocapError(-1, f"{what}: a blob with a hole is too large for the RETR_TREE slow path (wider or taller than 62 pixels, "
                              f"or more than 64 holes in the image); cv.findContours would give each hole a contour of its own "
-                             f"and fill the outer one (MOCAP_F_HOLES)")
+                             f"and fill the outer one (MOCAP_F_HOLES; large_holes=True lifts the size limit)")
     if flags:
         names = [n for b, n in _FLAG_NAMES.items() if flags & b]
         raise MocapError(-1, f"{what}: capacity overflow ({', '.join(names)}); results would be truncated "
@@ -88,6 +88,7 @@ class MocapContext:
         self.device = device
         self._tdev = None
         self._pp_in = None
+        self.large_holes = False
 
     # -- lifetime -------------------------------------------------------------------------
     def close(self):
@@ -116,6 +117,14 @@ class MocapContext:
         self._check(self.lib.mocap_set_stream(self.h, C.c_void_p(s.cuda_stream)))
 
     # -- session state --------------------------------------------------------------------
+    def set_large_holes(self, on=True):
+        """Reproduce cv.findContours(RETR_TREE) for holed blobs wider or taller than 62 pixels too (helpers.py:147-158),
+        in every S1 entry point of this context: a whole-image window for the slow path, about 166 KB of device memory
+        per SM at 640 x 480.  Off (the default) such an image keeps MOCAP_F_HOLES.  ``on=False`` frees the window
+        (mocap_set_large_holes, include/mocap_b200.h)."""
+        self._check(self.lib.mocap_set_large_holes(self.h, 1 if on else 0))
+        self.large_holes = bool(on)
+
     def set_cameras(self, intrinsics, poses):
         """intrinsics: C 3x3 matrices; poses: list of {"R": 3x3, "t": 3} as the reference passes them."""
         n = self.n_cam
@@ -644,9 +653,12 @@ class MocapSession:
 
     _default = None
 
-    def __init__(self, intrinsics, width=640, height=480, device=0):
+    def __init__(self, intrinsics, width=640, height=480, device=0, large_holes=False):
+        """``large_holes``: the contexts the session creates reproduce holed blobs wider or taller than 62 pixels as
+        cv2 does (MocapContext.set_large_holes); off, find_dot raises on a frame with one."""
         self.intrinsics = [np.asarray(k, dtype=np.float64).reshape(3, 3) for k in intrinsics]
         self.width, self.height, self.device = width, height, device
+        self.large_holes = bool(large_holes)
         self._ctxs = {}
         self._lock = threading.RLock()
 
@@ -665,7 +677,10 @@ class MocapSession:
         with self._lock:
             key = (n_cam, tuple(sorted(kw.items())))
             if key not in self._ctxs:
-                self._ctxs[key] = MocapContext(n_cam, self.width, self.height, self.device, **kw)
+                ctx = MocapContext(n_cam, self.width, self.height, self.device, **kw)
+                if self.large_holes:
+                    ctx.set_large_holes(True)
+                self._ctxs[key] = ctx
             return self._ctxs[key]
 
     def ctx_with_poses(self, camera_poses):
@@ -691,6 +706,8 @@ def find_dot(img, session=None):
         if ctx is None:
             ctx = MocapContext(1, w, h, s.device, max_blobs=MIRROR_LIMITS["max_blobs"],
                                max_segments=MIRROR_LIMITS["max_segments"])
+            if s.large_holes:
+                ctx.set_large_holes(True)
             s._ctxs[("detect", w, h)] = ctx
         d = ctx.detect(torch.from_numpy(img).to(ctx.torch_device))
         raise_on_overflow(d["flags"][0].item(), "find_dot")
@@ -903,7 +920,7 @@ PATCHED_NAMES = ("triangulate_point", "triangulate_points", "calculate_reproject
                  "bundle_adjustment", "locate_objects")
 
 
-def install_into(helpers_module, *also, session=None, tracker=False):
+def install_into(helpers_module, *also, session=None, tracker=False, large_holes=False):
     """Point a loaded reference ``helpers`` module at the CUDA path (INTEGRATION.md).
 
     ``also``: modules that imported the hot-path names BY VALUE -- the reference's ``index.py`` does
@@ -914,9 +931,15 @@ def install_into(helpers_module, *also, session=None, tracker=False):
 
     ``tracker=True`` also re-binds ``KalmanFilter`` (in helpers and in every module of ``also`` that holds it) to
     :class:`KalmanFilter` on this session, which ``start_trangulating_points`` (helpers.py:175) looks up at call
-    time; the default leaves the reference's CPU filter in place."""
+    time; the default leaves the reference's CPU filter in place.
+
+    ``large_holes=True``: the session made here reproduces holed blobs wider or taller than 62 pixels (a marker close to
+    a camera, which preprocessing turns into a ring; a lit fixture with dark spots) as cv2 does, at about 166 KB of
+    device memory per SM; by default ``_find_dot`` raises on such a frame.  A ``session`` passed in keeps its own
+    setting."""
     cams = helpers_module.Cameras.instance()
-    s = session or MocapSession.install([np.asarray(p["intrinsic_matrix"], dtype=np.float64) for p in cams.camera_params])
+    s = session or MocapSession.install([np.asarray(p["intrinsic_matrix"], dtype=np.float64) for p in cams.camera_params],
+                                        large_holes=large_holes)
     # helpers.Cameras is a Singleton WRAPPER object (Singleton.py:17-37); _camera_read looks _find_dot up on the
     # decorated class of the instance, so that is where the replacement goes
     type(cams)._find_dot = lambda self, img: find_dot(img, s)

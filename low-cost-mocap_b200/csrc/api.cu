@@ -142,6 +142,7 @@ void mocap_destroy(mocap_ctx* ctx) {
     cudaFree(ctx->d_seg_count); cudaFree(ctx->d_seg_list); cudaFree(ctx->d_worklist); cudaFree(ctx->d_work_count);
     cudaFree(ctx->d_set_worklist); cudaFree(ctx->d_img_done); cudaFree(ctx->d_set_done); cudaFree(ctx->d_unit_counter);
     cudaFree(ctx->d_blob_xy); cudaFree(ctx->d_blob_n); cudaFree(ctx->d_img_flags);
+    cudaFree(ctx->d_hole_win);
     cudaFree(ctx->d_stage[0]); cudaFree(ctx->d_stage[1]);
     cudaFree(ctx->d_obj); cudaFree(ctx->d_err); cudaFree(ctx->d_nobj); cudaFree(ctx->d_setflags);
     cudaFree(ctx->d_scratch);
@@ -163,6 +164,12 @@ int mocap_set_stream(mocap_ctx* ctx, void* cuda_stream) {
     if (!ctx) return MOCAP_EINVAL;
     ctx->stream = reinterpret_cast<cudaStream_t>(cuda_stream);
     return MOCAP_OK;
+}
+
+int mocap_set_large_holes(mocap_ctx* ctx, int on) {
+    if (!ctx) return MOCAP_EINVAL;
+    CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));
+    return blob_set_large_holes(ctx, on);
 }
 
 // ---- host-side camera tables: camera_tables.h ---------------------------------------------

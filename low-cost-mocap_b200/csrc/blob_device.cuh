@@ -144,6 +144,7 @@ struct BlobSmem {
     uint16_t* rowfirst;   // [row_cap] index of the first segment of row (rmin + k), 0xFFFF = empty; nullptr = binary search
     int row_cap;
     HoleScratch* hs;      // full-size (CTA) reduction only: scratch of the RETR_TREE slow path (blob_holes.cuh); else nullptr
+    unsigned long long* hole_win;   // this CTA's whole-image window in global memory (opt-in, blob_holes.cuh); nullptr: 64 x 64 only
 };
 // index of the first segment with position >= pos (pos lies in row pos / SPR): through the per-row index
 // when the image's rows fit it (one load + a scan over that row's few segments), else by binary search
@@ -173,6 +174,7 @@ __device__ __forceinline__ BlobSmem carve_blob_smem(unsigned char* raw, int E) {
     raw += (16 - (reinterpret_cast<uintptr_t>(raw) & 15)) & 15;
     s.hs = reinterpret_cast<HoleScratch*>(raw);
     s.rowfirst = nullptr; s.row_cap = 0;
+    s.hole_win = nullptr;
     return s;
 }
 
@@ -191,6 +193,100 @@ template <bool WIDE>
 __device__ __forceinline__ int acc_euler(const unsigned long long* acc, unsigned k) {
     const unsigned long long a3 = acc_get<WIDE>(acc, 4 * k + 3);
     return WIDE ? (int)(long long)(a3 >> 32) : ((int)((unsigned)a3 >> 20) << 20) >> 20;      // sign-extended
+}
+
+// RETR_TREE for holed blob k when it does not fit the 64 x 64 window and the whole-image window is on (blob_holes.cuh):
+// the steps of blob_holes_cta below, on sm.hole_win with the whole CTA.  Holes, parents and blob k's filled moments go
+// where blob_holes_cta keeps them; returns without a final barrier (the caller's).
+template <int NT, bool WIDE>
+__device__ __forceinline__ void blob_holes_wide(const BlobSmem& sm, unsigned k, unsigned n_runs, unsigned nb, int W, int H,
+                                                int x0, int y0, int w, int h) {
+    const int tid = threadIdx.x % NT;
+    const int SPR = W / MOCAP_SEG_PX;
+    HoleScratch& hs = *sm.hs;
+    const int nw = (w + 2 + 63) >> 6, nwords = (h + 2) * nw;
+    const size_t P = hole_wide_words(W, H);
+    unsigned long long *FS = sm.hole_win, *Ex = FS + P, *Hm = Ex + P, *Fh = Hm + P;
+    unsigned* flag = sm.wsum;                                            // [0..1] flood, [2] minimum, [4..11] four sums
+    unsigned long long* sums = reinterpret_cast<unsigned long long*>(sm.wsum + 4);
+    for (int i = tid; i < nwords; i += NT) { FS[i] = 0ull; Ex[i] = 0ull; Hm[i] = 0ull; Fh[i] = 0ull; }
+    __syncthreads();
+    for (unsigned id = tid; id < n_runs; id += NT) {                    // the blob's runs
+        if (sm.rank[sm.parent[id]] != k) continue;
+        const uint32_t p = sm.seg[sm.node_seg[id] & 0x7fff] >> 16;
+        const int y = p / SPR, sc = p - y * SPR;
+        const unsigned long long rb = sm.node_bits[id];
+        unsigned long long* row = FS + (size_t)(y - y0 + 1) * nw;
+        const int off = 16 * sc + 1 - x0;                               // window bit of the segment's pixel 0
+        if (off < 0) { atomicOr(&row[0], rb >> (-off)); continue; }
+        const int q = off >> 6, b = off & 63;
+        atomicOr(&row[q], rb << b);
+        if (b > 48 && (rb >> (64 - b))) atomicOr(&row[q + 1], rb >> (64 - b));
+    }
+    __syncthreads();
+    // the complement of the blob inside the window ("allowed"), and the exterior flood's seeds: the margin
+    const int wb = (w + 2) & 63;
+    const unsigned long long last = wb ? ((1ull << wb) - 1ull) : ~0ull;
+    const int qr = (w + 1) >> 6;
+    const unsigned long long br = 1ull << ((w + 1) & 63);
+    for (int i = tid; i < nwords; i += NT) {
+        const int r = i / nw, q = i - r * nw;
+        const unsigned long long fr = ~FS[i] & (q == nw - 1 ? last : ~0ull);
+        Hm[i] = fr;
+        Ex[i] = (r == 0 || r == h + 1) ? fr : (fr & ((q == 0 ? 1ull : 0ull) | (q == qr ? br : 0ull)));
+    }
+    __syncthreads();
+    hole_wide_flood<NT>(Ex, Hm, nw, h, tid, flag);
+    for (int i = tid; i < nwords; i += NT) Hm[i] &= ~Ex[i];            // what the outside does not reach
+    __syncthreads();
+    const long long sA2 = (long long)acc_get<WIDE>(sm.acc, 4 * k), sSX6 = (long long)acc_get<WIDE>(sm.acc, 4 * k + 1);
+    const long long sSY6 = (long long)acc_get<WIDE>(sm.acc, 4 * k + 2);
+    long long addA2 = 0, addSX6 = 0, addSY6 = 0;
+    const unsigned rowkey = 64u * (unsigned)nw;
+    while (true) {
+        // the first pixel, in raster order, of the regions still to be labelled: key = row * 64 nw + column
+        unsigned key = 0xffffffffu;
+        for (int r = tid; r <= h; r += NT)
+            for (int q = 0; q < nw; ++q) {
+                const unsigned long long m = Hm[(size_t)r * nw + q];
+                if (m) { key = min(key, (unsigned)r * rowkey + 64u * q + (unsigned)(__ffsll((long long)m) - 1)); break; }
+            }
+        key = cta_min_u32<NT>(key, flag + 2, tid);
+        if (key == 0xffffffffu) break;
+        const int j = hs.nholes;
+        if (j >= HOLE_CAP) { if (tid == 0) hs.unsupported = 1; break; }
+        const int r0 = (int)(key / rowkey), c0 = (int)(key - (unsigned)r0 * rowkey);
+        const int seed = r0 * nw + (c0 >> 6);
+        for (int i = tid; i < nwords; i += NT) Fh[i] = i == seed ? (1ull << (c0 & 63)) : 0ull;
+        __syncthreads();
+        hole_wide_flood<NT>(Fh, Hm, nw, h, tid, flag);
+        long long v[4] = {0, 0, 0, 0};
+        for (int i = tid; i < nwords; i += NT) { v[0] += __popcll(Fh[i]); Hm[i] &= ~Fh[i]; }
+        hole_wide_cellsum<NT>(FS, Fh, nw, h, tid, v[1], v[2], v[3]);
+        cta_sum4<NT>(v, sums, tid);
+        const long long size = v[0];
+        const long long hA2 = v[1] - sA2, hSX6 = v[2] + 3ll * (x0 - 1) * v[1] - sSX6, hSY6 = v[3] + 3ll * (y0 - 1) * v[1] - sSY6;
+        addA2 += hA2; addSX6 += hSX6; addSY6 += hSY6;
+        // blobs whose first pixel lies in this region: the innermost such region is their parent
+        for (unsigned t = tid; t < nb; t += NT) {
+            if (t == k) continue;
+            const int ty = (int)(hs.bfirst[t] / (uint32_t)W), tx = (int)(hs.bfirst[t] - (uint32_t)ty * (uint32_t)W);
+            const int wr = ty - y0 + 1, wc = tx - x0 + 1;
+            if (wr >= 0 && wr < h + 2 && wc >= 0 && wc < 64 * nw && ((Fh[(size_t)wr * nw + (wc >> 6)] >> (wc & 63)) & 1ull) &&
+                (uint32_t)size < hs.bbest[t]) {
+                hs.bbest[t] = (uint32_t)size; hs.bparent[t] = (int16_t)j;
+            }
+        }
+        if (tid == 0) {
+            hs.hA2[j] = hA2; hs.hSX6[j] = hSX6; hs.hSY6[j] = hSY6;
+            hs.hstart[j] = (uint32_t)((y0 - 1 + r0) * W + (x0 - 1 + c0)); hs.hsize[j] = (uint32_t)size; hs.hblob[j] = (uint16_t)k;
+            hs.nholes = j + 1;
+        }
+        __syncthreads();
+    }
+    if (tid == 0) {                                                      // the blob's outer contour runs around the FILLED blob
+        acc_add<WIDE>(sm.acc, 4 * k, addA2); acc_add<WIDE>(sm.acc, 4 * k + 1, addSX6); acc_add<WIDE>(sm.acc, 4 * k + 2, addSY6);
+    }
 }
 
 // RETR_TREE for an image that has a blob with a hole (see blob_holes.cuh).  Whole CTA; runs after the blobs' own
@@ -230,8 +326,9 @@ __device__ __noinline__ void blob_holes_cta(BlobSmem sm, int n, unsigned n_runs,
         }
         __syncthreads();
         const int x0 = hs.bbox[0], y0 = hs.bbox[1], w = hs.bbox[2] - x0 + 1, h = hs.bbox[3] - y0 + 1;
-        if (w + 2 > HOLE_WIN || h + 2 > HOLE_WIN) {                  // does not fit the window: left as the fast path has it
-            if (tid == 0) hs.unsupported = 1;
+        if (w + 2 > HOLE_WIN || h + 2 > HOLE_WIN) {                  // does not fit the window: left as the fast path has it,
+            if (sm.hole_win != nullptr) blob_holes_wide<NT, WIDE>(sm, k, n_runs, nb, W, H, x0, y0, w, h);   // or the whole-image one
+            else if (tid == 0) hs.unsupported = 1;
             __syncthreads();
             continue;
         }
@@ -336,21 +433,24 @@ __device__ __noinline__ void blob_holes_cta(BlobSmem sm, int n, unsigned n_runs,
         } else {
             // pre-order walk of the hierarchy without recursion: a frame lists either the blobs inside hole `owner`
             // (owner = -1: top level) or the holes of blob `owner`; siblings leave in descending order of their first
-            // pixel, found by scanning for the largest key below the one emitted last
-            struct Frame { int kind, owner; unsigned long long last; };
-            Frame st[34];
+            // pixel, found by scanning for the largest key below the one emitted last.  Keys are pixel indices, below
+            // W * H < 2^20 (mocap_create), so a frame fits 32 bits and the deepest nesting HOLE_CAP holes allow -- a blob
+            // and a hole frame per hole, plus two -- takes 520 bytes of stack
+            struct Frame { uint32_t last : 20, kind : 1, owner1 : 9; };        // owner1 = owner + 1; last 0xFFFFF: none yet
+            Frame st[2 * HOLE_CAP + 2];
             int sp = 0;
-            st[0].kind = 0; st[0].owner = -1; st[0].last = ~0ull;
+            st[0].last = 0xFFFFFu; st[0].kind = 0; st[0].owner1 = 0;
             while (sp >= 0) {
                 Frame& f = st[sp];
+                const int owner = (int)f.owner1 - 1;
                 int best = -1;
-                unsigned long long bkey = 0;
+                uint32_t bkey = 0;
                 if (f.kind == 0) {
                     for (int t = 0; t < (int)nb; ++t)
-                        if (hs.bparent[t] == f.owner && (unsigned long long)hs.bfirst[t] < f.last && (best < 0 || hs.bfirst[t] > bkey)) { best = t; bkey = hs.bfirst[t]; }
+                        if (hs.bparent[t] == owner && hs.bfirst[t] < f.last && (best < 0 || hs.bfirst[t] > bkey)) { best = t; bkey = hs.bfirst[t]; }
                 } else {
                     for (int j = 0; j < hs.nholes; ++j)
-                        if (hs.hblob[j] == f.owner && (unsigned long long)hs.hstart[j] < f.last && (best < 0 || hs.hstart[j] > bkey)) { best = j; bkey = hs.hstart[j]; }
+                        if (hs.hblob[j] == owner && hs.hstart[j] < f.last && (best < 0 || hs.hstart[j] > bkey)) { best = j; bkey = hs.hstart[j]; }
                 }
                 if (best < 0) { --sp; continue; }
                 f.last = bkey;
@@ -368,9 +468,9 @@ __device__ __noinline__ void blob_holes_cta(BlobSmem sm, int n, unsigned n_runs,
                     }
                     ++count;
                 }
-                if (sp + 1 < 34) {                                   // descend: a blob's holes, a hole's blobs
+                if (sp + 1 < 2 * HOLE_CAP + 2) {                     // descend: a blob's holes, a hole's blobs
                     ++sp;
-                    st[sp].kind = f.kind == 0 ? 1 : 0; st[sp].owner = best; st[sp].last = ~0ull;
+                    st[sp].last = 0xFFFFFu; st[sp].kind = f.kind == 0 ? 1 : 0; st[sp].owner1 = (uint32_t)(best + 1);
                 }
             }
             flags &= ~MOCAP_F_HOLES;

@@ -153,9 +153,11 @@ k_blob_reduce(uint32_t* __restrict__ seg_count, const uint32_t* __restrict__ seg
               int max_blobs, int32_t* __restrict__ blob_xy, int32_t* __restrict__ blob_n,
               int64_t* __restrict__ blob_mom, int32_t* __restrict__ img_flags,
               const uint32_t* __restrict__ worklist, uint32_t* __restrict__ work_count, uint32_t* __restrict__ done_count,
-              int stat_images, unsigned long long* __restrict__ stat_acc, unsigned long long* __restrict__ stat_host) {
+              int stat_images, unsigned long long* __restrict__ stat_acc, unsigned long long* __restrict__ stat_host,
+              unsigned long long* __restrict__ hole_win) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     BlobSmem sm = carve_blob_smem(smem_raw, E);
+    if (hole_win) sm.hole_win = hole_win + (size_t)blockIdx.x * 4 * hole_wide_words(W, H);     // mocap_set_large_holes
     const unsigned n_work = *work_count;
     for (unsigned w = blockIdx.x; w < n_work; w += gridDim.x) {
         const int img = (int)worklist[w];
@@ -275,12 +277,14 @@ int launch_blob_fallback(mocap_ctx* ctx, int32_t* blob_xy, int32_t* blob_n, int6
         k_blob_reduce<NT, true><<<grid2, NT, smem, ctx->stream>>>(ctx->d_seg_count, ctx->d_seg_list, E, c.width, c.height,
                                                                c.max_blobs, blob_xy, blob_n, blob_mom, img_flags,
                                                                ctx->d_worklist, ctx->d_work_count, ctx->d_work_count + 1,
-                                                               n_images, ctx->d_stat_acc, ctx->pipeline_auto ? ctx->d_stat_host : nullptr);
+                                                               n_images, ctx->d_stat_acc, ctx->pipeline_auto ? ctx->d_stat_host : nullptr,
+                                                               ctx->d_hole_win);
     else
         k_blob_reduce<NT, false><<<grid2, NT, smem, ctx->stream>>>(ctx->d_seg_count, ctx->d_seg_list, E, c.width, c.height,
                                                                 c.max_blobs, blob_xy, blob_n, blob_mom, img_flags,
                                                                 ctx->d_worklist, ctx->d_work_count, ctx->d_work_count + 1,
-                                                               n_images, ctx->d_stat_acc, ctx->pipeline_auto ? ctx->d_stat_host : nullptr);
+                                                               n_images, ctx->d_stat_acc, ctx->pipeline_auto ? ctx->d_stat_host : nullptr,
+                                                               ctx->d_hole_win);
     CUDA_TRY(ctx, cudaGetLastError());
     ctx->launches += 1;
     return MOCAP_OK;
@@ -295,6 +299,24 @@ int timing_flush(mocap_ctx* ctx) {
         ctx->detect_ms_n += 1;
     }
     ctx->tim_used = 0;
+    return MOCAP_OK;
+}
+
+// the whole-image window of the RETR_TREE slow path, one per CTA of k_blob_reduce (grid = num_sms): on = allocate, off = free
+int blob_set_large_holes(mocap_ctx* ctx, int on) {
+    if (!on == !ctx->d_hole_win) return MOCAP_OK;
+    CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));          // a k_blob_reduce in flight may still use the scratch
+    if (!on) {
+        CUDA_TRY(ctx, cudaFree(ctx->d_hole_win));
+        ctx->d_hole_win = nullptr;
+        return MOCAP_OK;
+    }
+    const size_t bytes = (size_t)ctx->num_sms * 4 * hole_wide_words(ctx->cfg.width, ctx->cfg.height) * sizeof(unsigned long long);
+    if (cudaMalloc(&ctx->d_hole_win, bytes) != cudaSuccess) {
+        cudaGetLastError();
+        ctx->d_hole_win = nullptr;
+        return mocap_fail(ctx, MOCAP_ENOMEM, "mocap_set_large_holes: %zu bytes of device memory for the whole-image windows", bytes);
+    }
     return MOCAP_OK;
 }
 

@@ -54,6 +54,7 @@ struct mocap_ctx {
     volatile unsigned long long* h_stat;             // pinned, mapped: {blobs, images} of the last batch, written by the GPU
     unsigned long long* d_stat_host;                 // device alias of h_stat
     int       use_fused;      // 1: single fused pipeline kernel for 1-channel frames (default)
+    unsigned long long* d_hole_win;   // mocap_set_large_holes: the whole-image windows of k_blob_reduce's CTAs; nullptr = off
     int32_t*  d_blob_xy;
     int32_t*  d_blob_n;
     int32_t*  d_img_flags;
@@ -105,6 +106,7 @@ int ensure_scratch(mocap_ctx* ctx, size_t bytes);
 int launch_locate(mocap_ctx* ctx, const double* obj, const double* err, const int32_t* n_obj, int n_sets,
                   int max_objects, double* out, int32_t* drone_index, int32_t* n_out);
 int launch_blob_fallback(mocap_ctx* ctx, int32_t* blob_xy, int32_t* blob_n, int64_t* blob_mom, int32_t* img_flags, int n_images);
+int blob_set_large_holes(mocap_ctx* ctx, int on);
 // frame-sets with more blobs than this (average of the previous batch) are cheaper through the three-kernel
 // pipeline: the matcher's large code then runs in a kernel of its own instead of evicting the stream loop
 #define MOCAP_HEAVY_BLOBS_PER_SET 48
