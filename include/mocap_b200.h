@@ -230,6 +230,63 @@ MOCAP_API int  mocap_track_objects_dev(mocap_tracker* tr, const double* objects,
                                        const int32_t* n_objects, int max_objects, const double* timestamps,
                                        int n_frame_sets, float* pos, float* vel, double* heading, uint8_t* present,
                                        int32_t* chosen);
+/* mocap_track_objects_dev with a gate: call uint8 [n_frame_sets] (DEVICE).  A frame-set whose call entry is 0 is not a
+ * predict_location call -- the reference makes none on a read where no camera saw a blob (helpers.py:90,106): the
+ * tracker's clock, call index and low-pass histories do not move, and its outputs are present = 0, chosen = -1 and
+ * zeros.  call == NULL: every frame-set is a call (= mocap_track_objects_dev). */
+MOCAP_API int  mocap_track_objects_gated_dev(mocap_tracker* tr, const double* objects, const int32_t* drone_index,
+                                             const int32_t* n_objects, int max_objects, const double* timestamps,
+                                             const uint8_t* call, int n_frame_sets, float* pos, float* vel, double* heading,
+                                             uint8_t* present, int32_t* chosen);
+
+/* The live capture loop -- replaces Cameras._camera_read (helpers.py:68-135) from the raw frames of the camera driver
+ * to the filtered drone states, for n_reads reads at once (a read is one call of _camera_read; n_reads = 1 in the
+ * live loop, more to replay a recorded session).  The context must have had mocap_set_preprocess; the read's chain is
+ * the existing stages: preprocessing -> S1 -> k_live_blobs (capture payload, gate, flags, dots) -> S2+S3 with the
+ * world transform -> locate_objects -> the gated tracker.
+ *   mode: bits of MOCAP_LIVE_*, following the reference's nesting (helpers.py:84-106): 0 = preprocessing only;
+ *   CAPTURE = S1 (needs no cameras: the reference has no poses yet in capture mode); CAPTURE|TRIANGULATE = also S2+S3
+ *   (needs mocap_set_cameras); CAPTURE|TRIANGULATE|LOCATE = also the locator and the tracker (needs tr, created on
+ *   this context, and timestamps).  Any other combination returns MOCAP_EINVAL before any launch.
+ *   raw uint8 [n_reads][n_cam][in_h][in_w][3]; timestamps double [n_reads] (the clock reading of each read, locate
+ *   mode only, may be NULL otherwise); frames uint8 [n_reads][n_cam][S][S][3] or NULL: the processed frames, with a
+ *   1-px (100, 255, 100) dot at every blob centre when CAPTURE is set (what the drop-in _find_dot draws).
+ *   result: ONE device buffer of mocap_live_layout(ctx, n_reads, tr ? num_objects : 0).total bytes, struct of arrays
+ *   over the reads, each slice written by the stage that computes it (byte offsets in mocap_live_layout):
+ *     flags      int32  [R]          OR of the read's images' MOCAP_F_* bits and its frame-set flags
+ *     gate       uint8  [R]          1 where some camera has at least one blob (helpers.py:90); 0 in mode 0
+ *     blob_n     int32  [R][C]       blobs per camera (0 in mode 0)
+ *     first      int32  [R][C][2]    first blob centre per camera, (-1, -1) if none (helpers.py:92)
+ *     n          int32  [R]          TRIANGULATE: points of the matcher (helpers.py:94)
+ *     obj        double [R][RM][3]   ... in world coordinates when a world transform is set (helpers.py:96-103)
+ *     err        double [R][RM]
+ *     n_objects  int32  [R]          LOCATE: locate_objects (helpers.py:105), M = max_roots records per read
+ *     objects    double [R][M][5]    {x, y, z, heading, error}
+ *     drone_index int32 [R][M]
+ *     called     uint8  [R]          LOCATE: 1 where the read is a predict_location call (= gate)
+ *     pos        float  [R][D][3]    LOCATE: the tracker's outputs (mocap_track_objects_gated_dev with call = called)
+ *     vel        float  [R][D][3]
+ *     heading    double [R][D]
+ *     present    uint8  [R][D]
+ *     chosen     int32  [R][D]
+ *   Slices a mode does not compute, and record slots beyond n / n_objects, are left unwritten.  DEVICE pointers,
+ *   never synchronises, allocates only while the context's scratch grows to the batch size. */
+#define MOCAP_LIVE_CAPTURE     1
+#define MOCAP_LIVE_TRIANGULATE 2
+#define MOCAP_LIVE_LOCATE      4
+typedef struct mocap_live_offsets {
+    uint64_t flags, gate, blob_n, first, n, obj, err, n_objects, objects, drone_index, called, pos, vel, heading, present,
+             chosen;
+    uint64_t total;     /* bytes of the result buffer; every slice starts on a 16-byte boundary */
+} mocap_live_offsets;
+MOCAP_API int  mocap_live_layout(mocap_ctx* ctx, int n_reads, int num_objects, mocap_live_offsets* layout);
+MOCAP_API int  mocap_live_dev(mocap_ctx* ctx, mocap_tracker* tr, const uint8_t* raw, int n_reads, int mode,
+                              const double* timestamps, uint8_t* frames, void* result);
+/* The same with HOST raw / timestamps / frames / result: one host-to-device copy (timestamps and raw frames through
+ * page-locked staging the context owns), the device chain, one device-to-host copy of the result and one of the frames
+ * (if asked for), one synchronisation. */
+MOCAP_API int  mocap_live_host(mocap_ctx* ctx, mocap_tracker* tr, const uint8_t* raw, int n_reads, int mode,
+                               const double* timestamps, uint8_t* frames, void* result);
 
 /* S3 -- replaces triangulate_points (helpers.py:330-336) and
  * calculate_reprojection_errors (helpers.py:203-211) on explicit correspondences.

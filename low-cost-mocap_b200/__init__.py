@@ -22,4 +22,6 @@ from .api import (  # noqa: F401
     install_into,
     KalmanFilter,
     Tracker,
+    camera_read,
+    live_read_events,
 )

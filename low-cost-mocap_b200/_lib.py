@@ -56,6 +56,14 @@ class BAProblem(C.Structure):
                 ("R", C.c_void_p), ("t", C.c_void_p), ("report", C.c_void_p)]
 
 
+LIVE_SLICES = ("flags", "gate", "blob_n", "first", "n", "obj", "err", "n_objects", "objects", "drone_index", "called", "pos",
+               "vel", "heading", "present", "chosen")
+
+
+class LiveLayout(C.Structure):
+    _fields_ = [(name, C.c_uint64) for name in LIVE_SLICES] + [("total", C.c_uint64)]
+
+
 MOCAP_BA_MAX_BATCH = 16
 
 # every symbol include/mocap_b200.h declares: name -> (restype, argtypes)
@@ -102,6 +110,10 @@ SYMBOLS = {
     "mocap_tracker_destroy": (None, [_P]),
     "mocap_tracker_reset": (C.c_int, [_P, C.c_double]),
     "mocap_track_objects_dev": (C.c_int, [_P, _P, _P, _P, C.c_int, _P, C.c_int, _P, _P, _P, _P, _P]),
+    "mocap_track_objects_gated_dev": (C.c_int, [_P, _P, _P, _P, C.c_int, _P, _P, C.c_int, _P, _P, _P, _P, _P]),
+    "mocap_live_layout": (C.c_int, [_P, C.c_int, C.c_int, C.POINTER(LiveLayout)]),
+    "mocap_live_dev": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P, _P, _P]),
+    "mocap_live_host": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P, _P, _P]),
     "mocap_ba_residuals_host": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, _P, _P, C.POINTER(C.c_int)]),
     "mocap_host_alloc": (C.c_int, [C.POINTER(_P), C.c_uint64]),
     "mocap_host_free": (None, [_P]),

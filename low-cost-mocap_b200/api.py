@@ -16,13 +16,14 @@ function raises :class:`MocapError` when the library or the GPU is missing.
 from __future__ import annotations
 
 import ctypes as C
+import json
 import threading
 import time
 
 import numpy as np
 
 from . import _lib
-from ._lib import MocapError, Config, BAOptions, BAProblem, BAReport, RansacOptions, GraphOptions, GraphPair, check
+from ._lib import MocapError, Config, BAOptions, BAProblem, BAReport, RansacOptions, GraphOptions, GraphPair, LiveLayout, check
 
 THRESHOLD = 51   # cv.threshold(grey, 255*0.2, 255, THRESH_BINARY) on uint8 == pix > 51 (helpers.py:146)
 
@@ -30,6 +31,9 @@ THRESHOLD = 51   # cv.threshold(grey, 255*0.2, 255, THRESH_BINARY) on uint8 == p
 F_SEGMENTS, F_BLOBS, F_ROOTS, F_CANDS, F_GROUPS, F_HOLES = 1, 2, 4, 8, 16, 32
 _FLAG_NAMES = {F_SEGMENTS: "max_segments", F_BLOBS: "max_blobs", F_ROOTS: "max_roots", F_CANDS: "max_cands",
                F_GROUPS: "max_groups"}
+# mode bits of mocap_live_dev (include/mocap_b200.h): Cameras.is_capturing_points, is_triangulating_points,
+# is_locating_objects, as the reference nests them (helpers.py:84-106)
+LIVE_CAPTURE, LIVE_TRIANGULATE, LIVE_LOCATE = 1, 2, 4
 # the reference is unbounded; the drop-in mirrors run with the compile-time maxima and raise on overflow
 MIRROR_LIMITS = dict(max_blobs=64, max_segments=4096, max_roots=128, max_cands=16, max_groups=1 << 16)
 
@@ -174,6 +178,75 @@ class MocapContext:
         self.use_current_stream()
         self._check(self.lib.mocap_pipeline_raw_dev(self.h, _ptr(raw.contiguous()), B, int(threshold), _ptr(frames),
                                                     _ptr(out["obj"]), _ptr(out["err"]), _ptr(out["n"]), _ptr(out["flags"])))
+        if want_frames:
+            out["frames"] = frames
+        return out
+
+    # -- the live capture loop (helpers.py:68-135) ---------------------------------------------
+    def live_layout(self, n_reads, num_objects=0):
+        """Byte offsets of the slices of a mocap_live_dev result buffer and its size (``total``)."""
+        L = LiveLayout()
+        self._check(self.lib.mocap_live_layout(self.h, int(n_reads), int(num_objects), C.byref(L)))
+        return L
+
+    def _live_views(self, buf, n_reads, num_objects, frombuffer):
+        """The result buffer's slices as arrays of their dtypes and shapes (views, no copy)."""
+        B, Cn, RM, D = n_reads, self.n_cam, self.cfg.max_roots, num_objects
+        L = self.live_layout(B, D)
+        spec = dict(flags=("int32", (B,)), gate=("uint8", (B,)), blob_n=("int32", (B, Cn)), first=("int32", (B, Cn, 2)),
+                    n=("int32", (B,)), obj=("float64", (B, RM, 3)), err=("float64", (B, RM)), n_objects=("int32", (B,)),
+                    objects=("float64", (B, RM, 5)), drone_index=("int32", (B, RM)), called=("uint8", (B,)),
+                    pos=("float32", (B, D, 3)), vel=("float32", (B, D, 3)), heading=("float64", (B, D)),
+                    present=("uint8", (B, D)), chosen=("int32", (B, D)))
+        return {k: frombuffer(buf, getattr(L, k), dt, shape) for k, (dt, shape) in spec.items()}
+
+    def _live_args(self, raw, mode, timestamps, tracker):
+        if self._pp_in is None:
+            raise MocapError(-5, "mocap_set_preprocess has not been called (MocapContext.set_preprocess)")
+        h, w = self._pp_in
+        per = self.n_cam * h * w * 3
+        n = raw.numel() if hasattr(raw, "numel") else raw.size
+        if n % per:
+            raise ValueError(f"raw must hold whole reads of {self.n_cam} x {h} x {w} x 3 bytes")
+        B = n // per
+        if mode & LIVE_LOCATE and (timestamps is None or len(timestamps) != B):
+            raise ValueError("locate mode needs one timestamp per read")
+        return B, (tracker.num_objects if tracker is not None else 0)
+
+    def live(self, raw, mode, timestamps=None, tracker=None, want_frames=False):
+        """The live capture loop for a batch of reads on the device (mocap_live_dev): raw uint8 cuda [B, C, in_h, in_w, 3],
+        mode a set of LIVE_* bits, timestamps f64 cuda [B] (locate mode), tracker a :class:`Tracker` of this context.
+        Returns a dict of views into one result buffer (``"buffer"``) -- flags, gate, blob_n, first, n, obj, err,
+        n_objects, objects, drone_index, called, pos, vel, heading, present, chosen; slices the mode does not compute
+        are undefined -- and ``"frames"`` uint8 [B, C, S, S, 3] with ``want_frames``.  No synchronisation."""
+        torch = _torch()
+        B, D = self._live_args(raw, mode, timestamps, tracker)
+        buf = torch.empty((self.live_layout(B, D).total,), dtype=torch.uint8, device=raw.device)
+        frames = torch.empty((B, self.n_cam, self.height, self.width, 3), dtype=torch.uint8, device=raw.device) if want_frames else None
+        ts = None if timestamps is None else timestamps.contiguous()
+        self.use_current_stream()
+        self._check(self.lib.mocap_live_dev(self.h, tracker.h if tracker is not None else None, _ptr(raw.contiguous()), B, int(mode),
+                                            _ptr(ts), _ptr(frames), _ptr(buf)))
+        out = self._live_views(buf, B, D, lambda b, off, dt, shape: b[off:off + int(np.prod(shape)) * np.dtype(dt).itemsize]
+                               .view(getattr(torch, dt)).view(shape))
+        out["buffer"] = buf
+        if want_frames:
+            out["frames"] = frames
+        return out
+
+    def live_host(self, raw, mode, timestamps=None, tracker=None, want_frames=False):
+        """The same on host arrays (mocap_live_host): raw uint8 ndarray [B, C, in_h, in_w, 3], timestamps a sequence of B
+        floats; one copy in, one copy back of the result (and of the frames), one synchronisation.  Returns numpy views."""
+        raw = np.ascontiguousarray(raw, dtype=np.uint8)
+        B, D = self._live_args(raw, mode, timestamps, tracker)
+        buf = np.empty((self.live_layout(B, D).total,), dtype=np.uint8)
+        frames = np.empty((B, self.n_cam, self.height, self.width, 3), dtype=np.uint8) if want_frames else None
+        ts = None if timestamps is None else np.ascontiguousarray(timestamps, dtype=np.float64)
+        self._check(self.lib.mocap_live_host(self.h, tracker.h if tracker is not None else None, _np_ptr(raw), B, int(mode),
+                                             _np_ptr(ts), _np_ptr(frames), _np_ptr(buf)))
+        out = self._live_views(buf, B, D, lambda b, off, dt, shape: b[off:off + int(np.prod(shape)) * np.dtype(dt).itemsize]
+                               .view(dt).reshape(shape))
+        out["buffer"] = buf
         if want_frames:
             out["frames"] = frames
         return out
@@ -598,12 +671,14 @@ class Tracker:
         next batch: every drone re-initialises at its next present step; covariances and low-pass histories stay."""
         self.ctx._check(self.ctx.lib.mocap_tracker_reset(self.h, float(prev_time)))
 
-    def track_dev(self, located, timestamps, out=None):
+    def track_dev(self, located, timestamps, out=None, calls=None):
         """located: the dict ``MocapContext.locate_objects`` returns (objects f64 [B, M, 5], drone_index int32 [B, M],
         n int32 [B]); timestamps: f64 cuda tensor [B] (seconds, one per frame-set).  Returns dict of cuda tensors, per
         frame-set and drone: pos f32 [B, D, 3], vel f32 [B, D, 3] and heading f64 [B, D] (low-pass filtered), present
         uint8 [B, D] and chosen int32 [B, D] (the object row, -1 if absent); pos / vel / heading are 0 where present
-        is 0.  Two launches."""
+        is 0.  Two launches.  ``calls`` (uint8 cuda [B], optional): frame-sets where it is 0 are not predict_location
+        calls -- the filters' clock and histories do not move there and the drones are absent
+        (mocap_track_objects_gated_dev)."""
         torch = _torch()
         obj, di, n = located["objects"], located["drone_index"], located["n"]
         B, M = obj.shape[0], obj.shape[1]
@@ -618,9 +693,17 @@ class Tracker:
                    "present": torch.empty((B, D), dtype=torch.uint8, device=dev),
                    "chosen": torch.empty((B, D), dtype=torch.int32, device=dev)}
         self.ctx.use_current_stream()
-        self.ctx._check(self.ctx.lib.mocap_track_objects_dev(self.h, _ptr(obj.contiguous()), _ptr(di.contiguous()), _ptr(n.contiguous()),
-                                                             M, _ptr(timestamps.contiguous()), B, _ptr(out["pos"]), _ptr(out["vel"]),
-                                                             _ptr(out["heading"]), _ptr(out["present"]), _ptr(out["chosen"])))
+        if calls is None:
+            self.ctx._check(self.ctx.lib.mocap_track_objects_dev(self.h, _ptr(obj.contiguous()), _ptr(di.contiguous()), _ptr(n.contiguous()),
+                                                                 M, _ptr(timestamps.contiguous()), B, _ptr(out["pos"]), _ptr(out["vel"]),
+                                                                 _ptr(out["heading"]), _ptr(out["present"]), _ptr(out["chosen"])))
+            return out
+        if tuple(calls.shape) != (B,) or calls.dtype != torch.uint8:
+            raise ValueError("calls must be a uint8 tensor with one entry per frame-set")
+        self.ctx._check(self.ctx.lib.mocap_track_objects_gated_dev(self.h, _ptr(obj.contiguous()), _ptr(di.contiguous()), _ptr(n.contiguous()),
+                                                                   M, _ptr(timestamps.contiguous()), _ptr(calls.contiguous()), B,
+                                                                   _ptr(out["pos"]), _ptr(out["vel"]), _ptr(out["heading"]),
+                                                                   _ptr(out["present"]), _ptr(out["chosen"])))
         return out
 
 
@@ -660,6 +743,7 @@ class MocapSession:
         self.width, self.height, self.device = width, height, device
         self.large_holes = bool(large_holes)
         self._ctxs = {}
+        self._live = {}
         self._lock = threading.RLock()
 
     @classmethod
@@ -915,12 +999,135 @@ def calculate_camera_poses(image_points, socketio=None, session=None, robust=Fal
     return out
 
 
+def live_read_events(res, r, mode, drone_armed):
+    """What ``Cameras._camera_read`` emits for read ``r`` of a live result (``MocapContext.live_host``; numpy views):
+    returns (events, serial), events a list of (name, payload) for ``socketio.emit`` and serial the list of byte strings
+    the reference writes to the drone link (helpers.py:88-133).  Nothing when the gate is closed; ``image-points`` in
+    capture-only mode; ``object-points`` when triangulating, with the locator's objects and the filtered drones when
+    locating.  An armed drone's heading is rounded to 4 decimals in its serial record and in the emitted payload, an
+    unarmed one's is not (helpers.py:114).  A capacity flag of the read raises MocapError, as find_dot does."""
+    if mode & LIVE_CAPTURE:
+        raise_on_overflow(res["flags"][r], "camera_read")
+    if not (mode & LIVE_CAPTURE) or not res["gate"][r]:
+        return [], []
+    if not (mode & LIVE_TRIANGULATE):
+        first = res["first"][r]
+        return [("image-points", [[int(x), int(y)] if res["blob_n"][r, c] > 0 else [None, None] for c, (x, y) in enumerate(first)])], []
+    k = int(res["n"][r])
+    payload = {"object_points": res["obj"][r, :k].tolist(), "errors": res["err"][r, :k].tolist(), "objects": [], "filtered_objects": []}
+    serial = []
+    if mode & LIVE_LOCATE:
+        m = int(res["n_objects"][r])
+        rec = res["objects"][r]
+        payload["objects"] = [{"pos": rec[i, :3].tolist(), "heading": np.float64(rec[i, 3]), "error": np.float64(rec[i, 4]),
+                               "droneIndex": int(res["drone_index"][r, i])} for i in range(m)]
+        filtered = []
+        for d in np.flatnonzero(res["present"][r]):
+            d = int(d)
+            pos, vel, heading = res["pos"][r, d], res["vel"][r, d], np.float64(res["heading"][r, d])
+            if drone_armed[d]:
+                heading = round(heading, 4)
+                data = {"pos": [round(x, 4) for x in pos.tolist()] + [heading], "vel": [round(x, 4) for x in vel.tolist()]}
+                serial.append(f"{d}{json.dumps(data)}".encode("utf-8"))
+            filtered.append({"pos": pos.tolist(), "vel": vel.tolist(), "heading": heading, "droneIndex": d})
+        payload["filtered_objects"] = filtered
+    return [("object-points", payload)], serial
+
+
+class _LiveCameras:
+    """Device state of one ``Cameras`` object under :func:`camera_read`: the context, built from the first read, and
+    what was last sent to it."""
+
+    def __init__(self, ctx, raw_shape):
+        self.ctx, self.raw_shape = ctx, raw_shape
+        self.poses = self.world = None
+        self.tracker, self.filter_obj = None, None
+
+
+def _live_cameras(cams, s, frames):
+    st = s._live.get(id(cams))
+    C_ = int(cams.num_cameras)
+    shape = tuple(np.shape(frames[0]))
+    if st is not None and st.raw_shape == (C_,) + shape:
+        return st
+    if len(shape) != 3 or shape[2] != 3:
+        raise ValueError(f"camera_read: the driver's frames must be H x W x 3 (got {shape})")
+    in_h, in_w = shape[0], shape[1]
+    params = [cams.camera_params[c] for c in range(C_)]
+    rot = [int(p["rotation"]) % 4 for p in params]
+    if any(r not in (0, 2) for r in rot):
+        raise ValueError(f"camera_read: rotations {rot} -- only 0 and 2 are supported: a quarter turn makes the frame portrait, "
+                         f"which the reference's make_square cannot feather (mocap_set_preprocess)")
+    S = max(in_w, in_h)
+    ctx = MocapContext(C_, S, S, s.device, **MIRROR_LIMITS)
+    if s.large_holes:
+        ctx.set_large_holes(True)
+    ctx.set_preprocess(in_w, in_h, rot, [np.asarray(p["intrinsic_matrix"], dtype=np.float64) for p in params],
+                       [np.asarray(p["distortion_coef"], dtype=np.float64).reshape(-1)[:5] for p in params])
+    if st is not None:
+        st.ctx.close()
+    st = s._live[id(cams)] = _LiveCameras(ctx, (C_,) + shape)
+    return st
+
+
+def camera_read(cams, session=None, clock=time.time):
+    """Replacement of ``Cameras._camera_read(self)`` (helpers.py:68-135) on the device: ``cams.cameras.read()``, then
+    one ``live_host`` call whose mode follows ``is_capturing_points`` / ``is_triangulating_points`` /
+    ``is_locating_objects`` as the reference nests them, then the reference's emits and serial writes
+    (:func:`live_read_events`).  Returns the processed frames -- with the centre dots while capturing -- in the container
+    type the driver gave.  The context is built from ``camera_params`` and the first read's size; poses and the world
+    matrix are re-sent only when their values change; a new ``kalman_filter`` object (start_trangulating_points) starts
+    a fresh device tracker, which reads ``clock`` once per read.  The filter object itself is never called."""
+    s = session or MocapSession.default()
+    frames, _ = cams.cameras.read()
+    capture = bool(cams.is_capturing_points)
+    tri = capture and bool(cams.is_triangulating_points)
+    loc = tri and bool(cams.is_locating_objects)
+    mode = (LIVE_CAPTURE if capture else 0) | (LIVE_TRIANGULATE if tri else 0) | (LIVE_LOCATE if loc else 0)
+    with s._lock:
+        st = _live_cameras(cams, s, frames)
+        ctx = st.ctx
+        if tri:
+            poses = np.concatenate([np.concatenate([np.asarray(p["R"], dtype=np.float64).reshape(9), np.asarray(p["t"], dtype=np.float64).reshape(3)])
+                                    for p in cams.camera_poses])
+            if st.poses is None or not np.array_equal(st.poses, poses):
+                ctx.set_cameras([np.asarray(cams.camera_params[c]["intrinsic_matrix"], dtype=np.float64) for c in range(ctx.n_cam)],
+                                cams.camera_poses)
+                st.poses = poses
+            if cams.to_world_coords_matrix is None:
+                raise TypeError("camera_read: to_world_coords_matrix is None; the reference's world transform needs it (helpers.py:99)")
+            world = np.asarray(cams.to_world_coords_matrix, dtype=np.float64).reshape(4, 4)
+            if st.world is None or not np.array_equal(st.world, world):
+                ctx.set_world_transform(world)
+                st.world = world.copy()
+        tracker = None
+        if loc:
+            if st.tracker is None or cams.kalman_filter is not st.filter_obj:
+                if st.tracker is not None:
+                    st.tracker.close()
+                st.tracker, st.filter_obj = Tracker(ctx, int(cams.num_objects)), cams.kalman_filter
+            tracker = st.tracker
+        raw = np.stack([np.asarray(f, dtype=np.uint8) for f in frames])[None]
+        res = ctx.live_host(raw, mode, [float(clock())] if loc else None, tracker, want_frames=True)
+    events, serial = live_read_events(res, 0, mode, cams.drone_armed if loc else ())
+    for name, payload in events:
+        cams.socketio.emit(name, payload)
+    for line in serial:
+        with cams.serialLock:
+            cams.ser.write(line)
+            time.sleep(0.001)
+    out = res["frames"][0]
+    if isinstance(frames, np.ndarray):
+        return out
+    return type(frames)(out[c] for c in range(len(out))) if isinstance(frames, tuple) else [out[c] for c in range(len(out))]
+
+
 PATCHED_NAMES = ("triangulate_point", "triangulate_points", "calculate_reprojection_error",
                  "calculate_reprojection_errors", "find_point_correspondance_and_object_points",
                  "bundle_adjustment", "locate_objects")
 
 
-def install_into(helpers_module, *also, session=None, tracker=False, large_holes=False):
+def install_into(helpers_module, *also, session=None, tracker=False, large_holes=False, live=False):
     """Point a loaded reference ``helpers`` module at the CUDA path (INTEGRATION.md).
 
     ``also``: modules that imported the hot-path names BY VALUE -- the reference's ``index.py`` does
@@ -936,13 +1143,22 @@ def install_into(helpers_module, *also, session=None, tracker=False, large_holes
     ``large_holes=True``: the session made here reproduces holed blobs wider or taller than 62 pixels (a marker close to
     a camera, which preprocessing turns into a ring; a lit fixture with dark spots) as cv2 does, at about 166 KB of
     device memory per SM; by default ``_find_dot`` raises on such a frame.  A ``session`` passed in keeps its own
-    setting."""
+    setting.
+
+    ``live=True`` also replaces ``_camera_read`` on the decorated class with :func:`camera_read`: the whole read --
+    preprocessing, S1-S3, the world transform, locate_objects and the tracker -- in one device call per read, the
+    driver call, emits and serial writes staying in Python."""
     cams = helpers_module.Cameras.instance()
     s = session or MocapSession.install([np.asarray(p["intrinsic_matrix"], dtype=np.float64) for p in cams.camera_params],
                                         large_holes=large_holes)
     # helpers.Cameras is a Singleton WRAPPER object (Singleton.py:17-37); _camera_read looks _find_dot up on the
     # decorated class of the instance, so that is where the replacement goes
     type(cams)._find_dot = lambda self, img: find_dot(img, s)
+    if live:
+        def _camera_read(self):
+            return camera_read(self, s)
+        _camera_read.__mocap_b200__ = True
+        type(cams)._camera_read = _camera_read
     repl = {
         "triangulate_point": lambda ip, cp: triangulate_point(ip, cp, s),
         "triangulate_points": lambda ip, cp: triangulate_points(ip, cp, s),

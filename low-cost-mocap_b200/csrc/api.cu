@@ -34,6 +34,47 @@ int ensure_scratch(mocap_ctx* ctx, size_t bytes) {
 }
 
 
+// ---- scratch management ------------------------------------------------------------------
+int ensure_images(mocap_ctx* ctx, int n_images) {
+    if (n_images <= ctx->cap_images) return MOCAP_OK;
+    CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+    cudaFree(ctx->d_seg_count); cudaFree(ctx->d_seg_list); cudaFree(ctx->d_worklist); cudaFree(ctx->d_work_count); cudaFree(ctx->d_set_worklist); cudaFree(ctx->d_img_done); cudaFree(ctx->d_set_done); cudaFree(ctx->d_unit_counter); cudaFree(ctx->d_blob_xy); cudaFree(ctx->d_blob_n); cudaFree(ctx->d_img_flags);
+    ctx->d_seg_count = nullptr; ctx->d_seg_list = nullptr; ctx->d_worklist = nullptr; ctx->d_work_count = nullptr; ctx->d_set_worklist = nullptr; ctx->d_img_done = nullptr; ctx->d_set_done = nullptr; ctx->d_unit_counter = nullptr; ctx->d_blob_xy = nullptr; ctx->d_blob_n = nullptr; ctx->d_img_flags = nullptr;
+    ctx->cap_images = 0;
+    const size_t n = (size_t)n_images;
+    CUDA_TRY(ctx, cudaMalloc(&ctx->d_seg_count, n * sizeof(uint32_t)));
+    CUDA_TRY(ctx, cudaMalloc(&ctx->d_seg_list, n * ctx->cfg.max_segments * sizeof(uint32_t)));
+    CUDA_TRY(ctx, cudaMalloc(&ctx->d_worklist, n * sizeof(uint32_t)));
+    CUDA_TRY(ctx, cudaMalloc(&ctx->d_work_count, 4 * sizeof(uint32_t)));
+    CUDA_TRY(ctx, cudaMemsetAsync(ctx->d_work_count, 0, 4 * sizeof(uint32_t), ctx->stream));
+    CUDA_TRY(ctx, cudaMalloc(&ctx->d_set_worklist, n * sizeof(uint32_t)));
+    CUDA_TRY(ctx, cudaMalloc(&ctx->d_img_done, n * sizeof(uint32_t)));
+    CUDA_TRY(ctx, cudaMalloc(&ctx->d_set_done, 2 * n * sizeof(uint32_t)));
+    CUDA_TRY(ctx, cudaMalloc(&ctx->d_unit_counter, sizeof(unsigned long long)));
+    CUDA_TRY(ctx, cudaMemsetAsync(ctx->d_img_done, 0, n * sizeof(uint32_t), ctx->stream));
+    CUDA_TRY(ctx, cudaMemsetAsync(ctx->d_set_done, 0, 2 * n * sizeof(uint32_t), ctx->stream));
+    CUDA_TRY(ctx, cudaMalloc(&ctx->d_blob_xy, n * ctx->cfg.max_blobs * 2 * sizeof(int32_t)));
+    CUDA_TRY(ctx, cudaMalloc(&ctx->d_blob_n, n * sizeof(int32_t)));
+    CUDA_TRY(ctx, cudaMalloc(&ctx->d_img_flags, n * sizeof(int32_t)));
+    CUDA_TRY(ctx, cudaMemsetAsync(ctx->d_seg_count, 0, n * sizeof(uint32_t), ctx->stream));   // kept zero by k_blob_reduce afterwards
+    ctx->cap_images = n_images;
+    return MOCAP_OK;
+}
+
+static int ensure_sets(mocap_ctx* ctx, int n_sets) {
+    if (n_sets <= ctx->cap_sets) return MOCAP_OK;
+    CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+    cudaFree(ctx->d_obj); cudaFree(ctx->d_err); cudaFree(ctx->d_nobj); cudaFree(ctx->d_setflags);
+    ctx->d_obj = nullptr; ctx->d_err = nullptr; ctx->d_nobj = nullptr; ctx->d_setflags = nullptr; ctx->cap_sets = 0;
+    const size_t n = (size_t)n_sets, R = ctx->cfg.max_roots;
+    CUDA_TRY(ctx, cudaMalloc(&ctx->d_obj, n * R * 3 * sizeof(double)));
+    CUDA_TRY(ctx, cudaMalloc(&ctx->d_err, n * R * sizeof(double)));
+    CUDA_TRY(ctx, cudaMalloc(&ctx->d_nobj, n * sizeof(int32_t)));
+    CUDA_TRY(ctx, cudaMalloc(&ctx->d_setflags, n * sizeof(int32_t)));
+    ctx->cap_sets = n_sets;
+    return MOCAP_OK;
+}
+
 extern "C" {
 
 const char* mocap_status_string(int status) {
@@ -150,6 +191,9 @@ void mocap_destroy(mocap_ctx* ctx) {
     cudaFree(ctx->d_match_counter);
     cudaFree(ctx->d_match_items); cudaFree(ctx->d_match_partial); cudaFree(ctx->d_match_range); cudaFree(ctx->d_match_arrive);
     cudaFree(ctx->d_pp_m1); cudaFree(ctx->d_pp_m2); cudaFree(ctx->d_pp_rot);
+    cudaFree(ctx->d_live_in); cudaFree(ctx->d_live_out);
+    if (ctx->h_live_in) cudaFreeHost(ctx->h_live_in);
+    if (ctx->h_live_out) cudaFreeHost(ctx->h_live_out);
     cudaFree(ctx->d_stat_acc);
     if (ctx->h_stat) cudaFreeHost(const_cast<unsigned long long*>(ctx->h_stat));
     if (ctx->copy_stream) cudaStreamDestroy(ctx->copy_stream);
@@ -209,47 +253,6 @@ static bool pick_fused(const mocap_ctx* ctx, int channels) {
     const unsigned long long blobs = ctx->h_stat[0], images = ctx->h_stat[1];
     if (images == 0) return true;
     return (double)blobs * ctx->cfg.n_cam <= (double)MOCAP_HEAVY_BLOBS_PER_SET * (double)images;
-}
-
-// ---- scratch management ------------------------------------------------------------------
-static int ensure_images(mocap_ctx* ctx, int n_images) {
-    if (n_images <= ctx->cap_images) return MOCAP_OK;
-    CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-    cudaFree(ctx->d_seg_count); cudaFree(ctx->d_seg_list); cudaFree(ctx->d_worklist); cudaFree(ctx->d_work_count); cudaFree(ctx->d_set_worklist); cudaFree(ctx->d_img_done); cudaFree(ctx->d_set_done); cudaFree(ctx->d_unit_counter); cudaFree(ctx->d_blob_xy); cudaFree(ctx->d_blob_n); cudaFree(ctx->d_img_flags);
-    ctx->d_seg_count = nullptr; ctx->d_seg_list = nullptr; ctx->d_worklist = nullptr; ctx->d_work_count = nullptr; ctx->d_set_worklist = nullptr; ctx->d_img_done = nullptr; ctx->d_set_done = nullptr; ctx->d_unit_counter = nullptr; ctx->d_blob_xy = nullptr; ctx->d_blob_n = nullptr; ctx->d_img_flags = nullptr;
-    ctx->cap_images = 0;
-    const size_t n = (size_t)n_images;
-    CUDA_TRY(ctx, cudaMalloc(&ctx->d_seg_count, n * sizeof(uint32_t)));
-    CUDA_TRY(ctx, cudaMalloc(&ctx->d_seg_list, n * ctx->cfg.max_segments * sizeof(uint32_t)));
-    CUDA_TRY(ctx, cudaMalloc(&ctx->d_worklist, n * sizeof(uint32_t)));
-    CUDA_TRY(ctx, cudaMalloc(&ctx->d_work_count, 4 * sizeof(uint32_t)));
-    CUDA_TRY(ctx, cudaMemsetAsync(ctx->d_work_count, 0, 4 * sizeof(uint32_t), ctx->stream));
-    CUDA_TRY(ctx, cudaMalloc(&ctx->d_set_worklist, n * sizeof(uint32_t)));
-    CUDA_TRY(ctx, cudaMalloc(&ctx->d_img_done, n * sizeof(uint32_t)));
-    CUDA_TRY(ctx, cudaMalloc(&ctx->d_set_done, 2 * n * sizeof(uint32_t)));
-    CUDA_TRY(ctx, cudaMalloc(&ctx->d_unit_counter, sizeof(unsigned long long)));
-    CUDA_TRY(ctx, cudaMemsetAsync(ctx->d_img_done, 0, n * sizeof(uint32_t), ctx->stream));
-    CUDA_TRY(ctx, cudaMemsetAsync(ctx->d_set_done, 0, 2 * n * sizeof(uint32_t), ctx->stream));
-    CUDA_TRY(ctx, cudaMalloc(&ctx->d_blob_xy, n * ctx->cfg.max_blobs * 2 * sizeof(int32_t)));
-    CUDA_TRY(ctx, cudaMalloc(&ctx->d_blob_n, n * sizeof(int32_t)));
-    CUDA_TRY(ctx, cudaMalloc(&ctx->d_img_flags, n * sizeof(int32_t)));
-    CUDA_TRY(ctx, cudaMemsetAsync(ctx->d_seg_count, 0, n * sizeof(uint32_t), ctx->stream));   // kept zero by k_blob_reduce afterwards
-    ctx->cap_images = n_images;
-    return MOCAP_OK;
-}
-
-static int ensure_sets(mocap_ctx* ctx, int n_sets) {
-    if (n_sets <= ctx->cap_sets) return MOCAP_OK;
-    CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-    cudaFree(ctx->d_obj); cudaFree(ctx->d_err); cudaFree(ctx->d_nobj); cudaFree(ctx->d_setflags);
-    ctx->d_obj = nullptr; ctx->d_err = nullptr; ctx->d_nobj = nullptr; ctx->d_setflags = nullptr; ctx->cap_sets = 0;
-    const size_t n = (size_t)n_sets, R = ctx->cfg.max_roots;
-    CUDA_TRY(ctx, cudaMalloc(&ctx->d_obj, n * R * 3 * sizeof(double)));
-    CUDA_TRY(ctx, cudaMalloc(&ctx->d_err, n * R * sizeof(double)));
-    CUDA_TRY(ctx, cudaMalloc(&ctx->d_nobj, n * sizeof(int32_t)));
-    CUDA_TRY(ctx, cudaMalloc(&ctx->d_setflags, n * sizeof(int32_t)));
-    ctx->cap_sets = n_sets;
-    return MOCAP_OK;
 }
 
 // ---- S1 ------------------------------------------------------------------------------------

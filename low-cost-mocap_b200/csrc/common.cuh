@@ -76,6 +76,9 @@ struct mocap_ctx {
     int32_t*  track_xy_cur;   // set for the duration of mocap_pipeline_tracks_dev: where the matcher leaves the winners' pixels
     // capture-side preprocessing (SURVEY 8(f) #2)
     int16_t*  d_pp_m1; uint16_t* d_pp_m2; int* d_pp_rot; int pp_in_w, pp_in_h;
+    // mocap_live_host staging: device and page-locked host buffers of {timestamps, raw frames} and {result, frames}
+    uint8_t*  d_live_in; uint8_t* h_live_in; size_t live_in_bytes;
+    uint8_t*  d_live_out; uint8_t* h_live_out; size_t live_out_bytes;
     // accounting
     uint64_t  launches;
     int       timing_on;
@@ -103,6 +106,20 @@ int launch_match(mocap_ctx* ctx, const int32_t* blob_xy, const int32_t* blob_n, 
 int launch_triangulate(mocap_ctx* ctx, const double* obs, const uint8_t* mask, int n_points,
                        const double* X_in, double* X, double* err, uint8_t* valid);
 int ensure_scratch(mocap_ctx* ctx, size_t bytes);
+int ensure_images(mocap_ctx* ctx, int n_images);
+// the live loop's per-read outputs k_live_blobs writes (slices of the mocap_live_dev result, indexed by read)
+struct LiveOut {
+    int32_t* flags; uint8_t* gate; int32_t* blob_n; int32_t* first; uint8_t* called;
+    int mode;                   // MOCAP_LIVE_* bits
+};
+int launch_live_blobs(mocap_ctx* ctx, const LiveOut& live, int s0, int n_sets, int have_blobs, uint8_t* frames);
+// raw frames -> preprocessing [-> S1 [-> S2+S3]] per launch group (preproc.cu)
+enum { RAW_PREPROCESS = 0, RAW_DETECT = 1, RAW_MATCH = 2 };
+int run_raw_groups(mocap_ctx* ctx, const uint8_t* raw_frames, int n_frame_sets, int threshold, int stages, uint8_t* processed,
+                   double* obj, double* err, int32_t* n_obj, int32_t* set_flags, const LiveOut* live);
+// the context and drone count of a tracker (track.cu)
+mocap_ctx* tracker_context(const mocap_tracker* tr);
+int tracker_num_objects(const mocap_tracker* tr);
 int launch_locate(mocap_ctx* ctx, const double* obj, const double* err, const int32_t* n_obj, int n_sets,
                   int max_objects, double* out, int32_t* drone_index, int32_t* n_out);
 int launch_blob_fallback(mocap_ctx* ctx, int32_t* blob_xy, int32_t* blob_n, int64_t* blob_mom, int32_t* img_flags, int n_images);

@@ -101,6 +101,58 @@ static void build_undistort_map(const double* K, const double* dist, int S, int1
     }
 }
 
+// processed frames and/or the grayscale plane S1 derives from them
+static int launch_preprocess(mocap_ctx* ctx, const uint8_t* raw_frames, int n_images, uint8_t* out_frames, uint8_t* gray) {
+    const int S = ctx->cfg.width, C = ctx->cfg.n_cam;
+    const int groups_per_launch = 65535 / C > 0 ? 65535 / C : 1;           // gridDim.z <= 65535
+    const int per_launch = groups_per_launch * PP_F * C;                    // whole frame-sets, whole groups
+    for (int i0 = 0; i0 < n_images; i0 += per_launch) {
+        const int n = n_images - i0 < per_launch ? n_images - i0 : per_launch;
+        const int sets = (n + C - 1) / C, groups = (sets + PP_F - 1) / PP_F;
+        uint8_t* o = out_frames ? out_frames + (size_t)i0 * S * S * 3 : nullptr;
+        uint8_t* g = gray ? gray + (size_t)i0 * S * S : nullptr;
+        const int word_stores = (S % 4 == 0) && (reinterpret_cast<uintptr_t>(o) % 4 == 0) && (reinterpret_cast<uintptr_t>(g) % 4 == 0);
+        k_preprocess<<<dim3((S + PP_TX - 1) / PP_TX, (S + PP_TY - 1) / PP_TY, groups * C), 256, 0, ctx->stream>>>(
+            raw_frames + (size_t)i0 * ctx->pp_in_w * ctx->pp_in_h * 3, n, C, ctx->pp_in_w, ctx->pp_in_h, S, ctx->d_pp_rot,
+            reinterpret_cast<const int32_t*>(ctx->d_pp_m1), ctx->d_pp_m2, o, g, word_stores);
+        CUDA_TRY(ctx, cudaGetLastError());
+        ctx->launches += 1;
+    }
+    return MOCAP_OK;
+}
+
+// The launch-group loop of the raw-frame entry points (mocap_pipeline_raw_dev, mocap_live_dev).  The preprocessing
+// kernel also emits the grayscale plane _find_dot would derive from the processed frame (helpers.py:144), so S1-S3 run
+// on 1 byte per pixel through the single-pass pipeline kernel; the processed BGR frames are only written when the
+// caller asks for them.  stages: RAW_PREPROCESS, RAW_DETECT (+ S1, blob lists left in the context's d_blob_xy /
+// d_blob_n / d_img_flags) or RAW_MATCH (+ S2+S3 into obj / err / n_obj / set_flags, the blob lists left as well).
+// live != NULL: k_live_blobs after each group's S1 (live.cu).
+int run_raw_groups(mocap_ctx* ctx, const uint8_t* raw_frames, int n_frame_sets, int threshold, int stages, uint8_t* processed,
+                   double* obj, double* err, int32_t* n_obj, int32_t* set_flags, const LiveOut* live) {
+    const int C = ctx->cfg.n_cam, S = ctx->cfg.width;
+    const size_t gray_bytes = (size_t)S * S;
+    const int chunk = 4096 / C > 0 ? 4096 / C : 1;             // frame-sets per launch group (bounded scratch)
+    int st = ensure_scratch(ctx, (size_t)chunk * C * gray_bytes);
+    if (st) return st;
+    if (stages == RAW_DETECT && (st = ensure_images(ctx, (n_frame_sets < chunk ? n_frame_sets : chunk) * C)) != MOCAP_OK) return st;
+    uint8_t* gray = static_cast<uint8_t*>(ctx->d_scratch);
+    for (int s0 = 0; s0 < n_frame_sets; s0 += chunk) {
+        const int ns = n_frame_sets - s0 < chunk ? n_frame_sets - s0 : chunk;
+        uint8_t* out = processed ? processed + (size_t)s0 * C * gray_bytes * 3 : nullptr;
+        st = launch_preprocess(ctx, raw_frames + (size_t)s0 * C * ctx->pp_in_w * ctx->pp_in_h * 3, ns * C, out,
+                               stages == RAW_PREPROCESS ? nullptr : gray);
+        if (st) return st;
+        if (stages == RAW_MATCH)
+            st = mocap_pipeline_dev(ctx, gray, ns, 1, threshold, obj + (size_t)s0 * ctx->cfg.max_roots * 3, err + (size_t)s0 * ctx->cfg.max_roots,
+                                    n_obj + s0, set_flags ? set_flags + s0 : nullptr);
+        else if (stages == RAW_DETECT)
+            st = launch_detect(ctx, gray, ns * C, 1, threshold, ctx->d_blob_xy, ctx->d_blob_n, nullptr, ctx->d_img_flags);
+        if (st) return st;
+        if (live && (st = launch_live_blobs(ctx, *live, s0, ns, stages != RAW_PREPROCESS, out)) != MOCAP_OK) return st;
+    }
+    return MOCAP_OK;
+}
+
 extern "C" {
 
 int mocap_set_preprocess(mocap_ctx* ctx, int in_width, int in_height, const int* rotation, const double* K, const double* dist) {
@@ -140,26 +192,6 @@ int mocap_get_undistort_map(mocap_ctx* ctx, int cam, int16_t* m1, uint16_t* m2) 
     return MOCAP_OK;
 }
 
-// processed frames and/or the grayscale plane S1 derives from them
-static int launch_preprocess(mocap_ctx* ctx, const uint8_t* raw_frames, int n_images, uint8_t* out_frames, uint8_t* gray) {
-    const int S = ctx->cfg.width, C = ctx->cfg.n_cam;
-    const int groups_per_launch = 65535 / C > 0 ? 65535 / C : 1;           // gridDim.z <= 65535
-    const int per_launch = groups_per_launch * PP_F * C;                    // whole frame-sets, whole groups
-    for (int i0 = 0; i0 < n_images; i0 += per_launch) {
-        const int n = n_images - i0 < per_launch ? n_images - i0 : per_launch;
-        const int sets = (n + C - 1) / C, groups = (sets + PP_F - 1) / PP_F;
-        uint8_t* o = out_frames ? out_frames + (size_t)i0 * S * S * 3 : nullptr;
-        uint8_t* g = gray ? gray + (size_t)i0 * S * S : nullptr;
-        const int word_stores = (S % 4 == 0) && (reinterpret_cast<uintptr_t>(o) % 4 == 0) && (reinterpret_cast<uintptr_t>(g) % 4 == 0);
-        k_preprocess<<<dim3((S + PP_TX - 1) / PP_TX, (S + PP_TY - 1) / PP_TY, groups * C), 256, 0, ctx->stream>>>(
-            raw_frames + (size_t)i0 * ctx->pp_in_w * ctx->pp_in_h * 3, n, C, ctx->pp_in_w, ctx->pp_in_h, S, ctx->d_pp_rot,
-            reinterpret_cast<const int32_t*>(ctx->d_pp_m1), ctx->d_pp_m2, o, g, word_stores);
-        CUDA_TRY(ctx, cudaGetLastError());
-        ctx->launches += 1;
-    }
-    return MOCAP_OK;
-}
-
 int mocap_preprocess_dev(mocap_ctx* ctx, const uint8_t* raw_frames, int n_images, uint8_t* out_frames) {
     if (!ctx) return MOCAP_EINVAL;
     if (!raw_frames || !out_frames || n_images < 0) return mocap_fail(ctx, MOCAP_EINVAL, "mocap_preprocess_dev: bad argument");
@@ -176,26 +208,8 @@ int mocap_pipeline_raw_dev(mocap_ctx* ctx, const uint8_t* raw_frames, int n_fram
     if (!ctx->d_pp_m1) return mocap_fail(ctx, MOCAP_ESTATE, "mocap_set_preprocess has not been called");
     if (!ctx->cameras_set) return mocap_fail(ctx, MOCAP_ESTATE, "mocap_set_cameras has not been called");
     if (n_frame_sets == 0) return MOCAP_OK;
-    const int C = ctx->cfg.n_cam, S = ctx->cfg.width;
     CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));
-    // The preprocessing kernel also emits the grayscale plane _find_dot would derive from the processed frame
-    // (helpers.py:144), so S1-S3 run on 1 byte per pixel through the single-pass pipeline kernel; the
-    // processed BGR frames are only written when the caller asks for them.
-    const size_t gray_bytes = (size_t)S * S;
-    const int chunk = 4096 / C > 0 ? 4096 / C : 1;             // frame-sets per launch group (bounded scratch)
-    int st = ensure_scratch(ctx, (size_t)chunk * C * gray_bytes);
-    if (st) return st;
-    uint8_t* gray = static_cast<uint8_t*>(ctx->d_scratch);
-    for (int s0 = 0; s0 < n_frame_sets; s0 += chunk) {
-        const int ns = n_frame_sets - s0 < chunk ? n_frame_sets - s0 : chunk;
-        st = launch_preprocess(ctx, raw_frames + (size_t)s0 * C * ctx->pp_in_w * ctx->pp_in_h * 3, ns * C,
-                               processed ? processed + (size_t)s0 * C * gray_bytes * 3 : nullptr, gray);
-        if (st) return st;
-        st = mocap_pipeline_dev(ctx, gray, ns, 1, threshold, obj + (size_t)s0 * ctx->cfg.max_roots * 3, err + (size_t)s0 * ctx->cfg.max_roots,
-                                n_obj + s0, set_flags ? set_flags + s0 : nullptr);
-        if (st) return st;
-    }
-    return MOCAP_OK;
+    return run_raw_groups(ctx, raw_frames, n_frame_sets, threshold, RAW_MATCH, processed, obj, err, n_obj, set_flags, nullptr);
 }
 
 }  // extern "C"

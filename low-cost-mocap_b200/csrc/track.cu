@@ -6,7 +6,8 @@
 //   ballot, split the 9 x 9 products of the predict / correct steps over the entries and the association over the
 //   candidates.  It writes pos, present and chosen, and appends the low-pass inputs of each present frame-set (the
 //   posterior velocity and the chosen object's heading) to the drone's history rows, which carry the last
-//   TRACK_HIST samples over to the next batch.  A pending reset is applied before the first frame-set.
+//   TRACK_HIST samples over to the next batch.  A pending reset is applied before the first frame-set.  A frame-set
+//   whose call entry is 0 (call != NULL) is skipped: absent outputs, and neither the clock nor the history moves.
 // k_track_lowpass: one thread per (frame-set, drone, channel); each runs its window of <= 300 samples from zero state.
 #include <math.h>
 #include "common.cuh"
@@ -26,7 +27,8 @@ struct mocap_tracker {
 __global__ void __launch_bounds__(32 * TRACK_MAX_DRONES)
 k_track_scan(TrackDrone* __restrict__ state, double* __restrict__ hist, int stride, const double* __restrict__ objects,
              const int32_t* __restrict__ drone_index, const int32_t* __restrict__ n_objects, int max_objects,
-             const double* __restrict__ timestamps, int n_sets, int reset, double reset_time, float* __restrict__ pos,
+             const double* __restrict__ timestamps, const uint8_t* __restrict__ call, int n_sets, int reset, double reset_time,
+             float* __restrict__ pos,
              uint8_t* __restrict__ present, int32_t* __restrict__ chosen, int2* __restrict__ slot) {
     __shared__ TrackWork work[TRACK_MAX_DRONES];
     __shared__ TrackDrone drones[TRACK_MAX_DRONES];
@@ -63,6 +65,12 @@ k_track_scan(TrackDrone* __restrict__ state, double* __restrict__ hist, int stri
     __syncwarp();
 
     for (int s = 0; s < n_sets; ++s) {
+        const size_t o = (size_t)s * D + d;
+        if (call && !call[s]) {
+            if (lane < 3) pos[3 * o + lane] = 0.0f;
+            if (lane == 0) { present[o] = 0; chosen[o] = -1; slot[o] = make_int2(0, 0); }
+            continue;
+        }
         const double t = timestamps[s];
         const double dt = DSUB(t, prev_time);
         prev_time = t;
@@ -74,7 +82,6 @@ k_track_scan(TrackDrone* __restrict__ state, double* __restrict__ hist, int stri
             const unsigned hit = __ballot_sync(0xffffffffu, c0 + lane < n && di[c0 + lane] == d);
             if (hit) first = c0 + __ffs(hit) - 1;
         }
-        const size_t o = (size_t)s * D + d;
         if (first < 0) {
             if (lane < 3) pos[3 * o + lane] = 0.0f;
             if (lane == 0) { present[o] = 0; chosen[o] = -1; slot[o] = make_int2(0, 0); }
@@ -144,6 +151,9 @@ k_track_lowpass(const double* __restrict__ hist, int stride, const int2* __restr
     if (ch < 3) vel[3 * o + ch] = TF32(y);
     else heading[o] = y;
 }
+
+mocap_ctx* tracker_context(const mocap_tracker* tr) { return tr->ctx; }
+int tracker_num_objects(const mocap_tracker* tr) { return tr->num_objects; }
 
 static size_t hist_stride(int cap) { return (size_t)TRACK_HIST + (size_t)cap; }
 
@@ -220,6 +230,13 @@ int mocap_tracker_reset(mocap_tracker* tr, double prev_time) {
 int mocap_track_objects_dev(mocap_tracker* tr, const double* objects, const int32_t* drone_index, const int32_t* n_objects,
                             int max_objects, const double* timestamps, int n_frame_sets, float* pos, float* vel,
                             double* heading, uint8_t* present, int32_t* chosen) {
+    return mocap_track_objects_gated_dev(tr, objects, drone_index, n_objects, max_objects, timestamps, nullptr, n_frame_sets, pos,
+                                         vel, heading, present, chosen);
+}
+
+int mocap_track_objects_gated_dev(mocap_tracker* tr, const double* objects, const int32_t* drone_index, const int32_t* n_objects,
+                                  int max_objects, const double* timestamps, const uint8_t* call, int n_frame_sets, float* pos,
+                                  float* vel, double* heading, uint8_t* present, int32_t* chosen) {
     if (!tr) return MOCAP_EINVAL;
     mocap_ctx* ctx = tr->ctx;
     if (!objects || !drone_index || !n_objects || !timestamps || !pos || !vel || !heading || !present || !chosen)
@@ -233,7 +250,7 @@ int mocap_track_objects_dev(mocap_tracker* tr, const double* objects, const int3
     const int D = tr->num_objects;
     const int stride = (int)hist_stride(tr->cap);
     k_track_scan<<<1, 32 * D, 0, ctx->stream>>>(tr->d_state, tr->d_hist, stride, objects, drone_index, n_objects, max_objects,
-                                                timestamps, n_frame_sets, tr->reset_pending, tr->reset_time, pos, present, chosen,
+                                                timestamps, call, n_frame_sets, tr->reset_pending, tr->reset_time, pos, present, chosen,
                                                 tr->d_slot);
     CUDA_TRY(ctx, cudaGetLastError());
     tr->reset_pending = 0;
