@@ -288,6 +288,30 @@ MOCAP_API int  mocap_live_dev(mocap_ctx* ctx, mocap_tracker* tr, const uint8_t* 
 MOCAP_API int  mocap_live_host(mocap_ctx* ctx, mocap_tracker* tr, const uint8_t* raw, int n_reads, int mode,
                                const double* timestamps, uint8_t* frames, void* result);
 
+/* Baseline JPEG encoding -- the camera stream's cv.imencode('.jpg', frames) (index.py:55-56), byte for byte what
+ * cv2.imencode('.jpg', img, [cv2.IMWRITE_JPEG_QUALITY, quality]) returns with libjpeg-turbo: 3-channel BGR input,
+ * 4:2:0, the standard (Annex K) Huffman tables, JFIF 1.01, no restart markers.
+ * mocap_jpeg_bound: worst-case bytes of one width x height image, header and EOI included (0 for a size outside
+ * 1..65500).
+ * mocap_encode_jpeg_dev: images uint8 [n_images][tile_h][tiles * tile_w][3], stored as the frames side by side are
+ *   stored one after another, [n_images][tiles][tile_h][tile_w][3] -- np.hstack of `tiles` frames without the copy;
+ *   tiles = 1 is a plain image.  out uint8 [n_images][out_stride]: image i's JPEG from out + i * out_stride;
+ *   out_len int32 [n_images]: its length, or -1 when it does not fit out_stride (then nothing of it is written).
+ *   quality 1..100; any other, n_images < 0, tiles, tile_w or tile_h < 1, or a side over 65500 give MOCAP_EINVAL before
+ *   any launch.  DEVICE pointers, the context's stream, never synchronises; 4 launches per group of images (a group is
+ *   as many as fit 256 MB of scratch, about 8 bytes per pixel).
+ * mocap_live_jpeg_host: mocap_live_host (same chain, same outputs), plus the JPEG of each read's processed frames side
+ *   by side (np.hstack, helpers.py:141; with the dots in capture mode) at `quality`: HOST jpeg uint8
+ *   [n_reads][jpeg_stride], jpeg_len int32 [n_reads]; frames may be NULL.  Copies back exactly the JPEG bytes.  Two
+ *   synchronisations: one for the result, the frames and the lengths, one for the bytes.  A JPEG longer than
+ *   jpeg_stride returns MOCAP_EINVAL after the first (jpeg is then not written; result and frames are). */
+MOCAP_API uint64_t mocap_jpeg_bound(int width, int height);
+MOCAP_API int  mocap_encode_jpeg_dev(mocap_ctx* ctx, const uint8_t* images, int n_images, int tiles, int tile_w, int tile_h,
+                                     int quality, uint8_t* out, uint64_t out_stride, int32_t* out_len);
+MOCAP_API int  mocap_live_jpeg_host(mocap_ctx* ctx, mocap_tracker* tr, const uint8_t* raw, int n_reads, int mode,
+                                    const double* timestamps, uint8_t* frames, void* result,
+                                    int quality, uint8_t* jpeg, uint64_t jpeg_stride, int32_t* jpeg_len);
+
 /* S3 -- replaces triangulate_points (helpers.py:330-336) and
  * calculate_reprojection_errors (helpers.py:203-211) on explicit correspondences.
  * obs double [n_points][n_cam][2], mask uint8 [n_points][n_cam] (0 = [None, None]).

@@ -24,4 +24,6 @@ from .api import (  # noqa: F401
     Tracker,
     camera_read,
     live_read_events,
+    StreamFrames,
+    StreamCv,
 )

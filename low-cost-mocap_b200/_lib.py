@@ -114,6 +114,9 @@ SYMBOLS = {
     "mocap_live_layout": (C.c_int, [_P, C.c_int, C.c_int, C.POINTER(LiveLayout)]),
     "mocap_live_dev": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P, _P, _P]),
     "mocap_live_host": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P, _P, _P]),
+    "mocap_jpeg_bound": (C.c_uint64, [C.c_int, C.c_int]),
+    "mocap_encode_jpeg_dev": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, C.c_uint64, _P]),
+    "mocap_live_jpeg_host": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P, _P, _P, C.c_int, _P, C.c_uint64, _P]),
     "mocap_ba_residuals_host": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, _P, _P, C.POINTER(C.c_int)]),
     "mocap_host_alloc": (C.c_int, [C.POINTER(_P), C.c_uint64]),
     "mocap_host_free": (None, [_P]),

@@ -34,6 +34,8 @@ _FLAG_NAMES = {F_SEGMENTS: "max_segments", F_BLOBS: "max_blobs", F_ROOTS: "max_r
 # mode bits of mocap_live_dev (include/mocap_b200.h): Cameras.is_capturing_points, is_triangulating_points,
 # is_locating_objects, as the reference nests them (helpers.py:84-106)
 LIVE_CAPTURE, LIVE_TRIANGULATE, LIVE_LOCATE = 1, 2, 4
+# cv2's default IMWRITE_JPEG_QUALITY, what index.py's cv.imencode('.jpg', frames) (index.py:56) encodes at
+JPEG_QUALITY = 95
 # the reference is unbounded; the drop-in mirrors run with the compile-time maxima and raise on overflow
 MIRROR_LIMITS = dict(max_blobs=64, max_segments=4096, max_roots=128, max_cands=16, max_groups=1 << 16)
 
@@ -234,22 +236,64 @@ class MocapContext:
             out["frames"] = frames
         return out
 
-    def live_host(self, raw, mode, timestamps=None, tracker=None, want_frames=False):
+    def live_host(self, raw, mode, timestamps=None, tracker=None, want_frames=False, jpeg=False, quality=JPEG_QUALITY,
+                  jpeg_stride=None):
         """The same on host arrays (mocap_live_host): raw uint8 ndarray [B, C, in_h, in_w, 3], timestamps a sequence of B
-        floats; one copy in, one copy back of the result (and of the frames), one synchronisation.  Returns numpy views."""
+        floats; one copy in, one copy back of the result (and of the frames), one synchronisation.  Returns numpy views.
+        ``jpeg=True`` (mocap_live_jpeg_host): also each read's processed frames side by side as cv2.imencode('.jpg')
+        encodes them at ``quality``, encoded on the device -- ``"jpeg"`` uint8 [B, jpeg_stride] (default: the worst
+        case) and ``"jpeg_len"`` int32 [B]; two synchronisations.  A JPEG longer than jpeg_stride raises MocapError."""
         raw = np.ascontiguousarray(raw, dtype=np.uint8)
         B, D = self._live_args(raw, mode, timestamps, tracker)
         buf = np.empty((self.live_layout(B, D).total,), dtype=np.uint8)
         frames = np.empty((B, self.n_cam, self.height, self.width, 3), dtype=np.uint8) if want_frames else None
         ts = None if timestamps is None else np.ascontiguousarray(timestamps, dtype=np.float64)
-        self._check(self.lib.mocap_live_host(self.h, tracker.h if tracker is not None else None, _np_ptr(raw), B, int(mode),
-                                             _np_ptr(ts), _np_ptr(frames), _np_ptr(buf)))
+        trh = tracker.h if tracker is not None else None
+        if jpeg:
+            stride = int(jpeg_stride if jpeg_stride is not None else self.lib.mocap_jpeg_bound(self.n_cam * self.width, self.height))
+            jbuf = np.empty((B, stride), dtype=np.uint8)
+            jlen = np.empty((B,), dtype=np.int32)
+            self._check(self.lib.mocap_live_jpeg_host(self.h, trh, _np_ptr(raw), B, int(mode), _np_ptr(ts), _np_ptr(frames), _np_ptr(buf),
+                                                      int(quality), _np_ptr(jbuf), stride, _np_ptr(jlen)))
+        else:
+            self._check(self.lib.mocap_live_host(self.h, trh, _np_ptr(raw), B, int(mode), _np_ptr(ts), _np_ptr(frames), _np_ptr(buf)))
         out = self._live_views(buf, B, D, lambda b, off, dt, shape: b[off:off + int(np.prod(shape)) * np.dtype(dt).itemsize]
                                .view(dt).reshape(shape))
         out["buffer"] = buf
         if want_frames:
             out["frames"] = frames
+        if jpeg:
+            out["jpeg"], out["jpeg_len"] = jbuf, jlen
         return out
+
+    # -- JPEG (the camera stream, index.py:55-56) ------------------------------------------------
+    def jpeg_bound(self, width, height):
+        """Worst-case bytes of the JPEG of one width x height image (mocap_jpeg_bound)."""
+        return int(self.lib.mocap_jpeg_bound(int(width), int(height)))
+
+    def encode_jpeg(self, images, tiles=1, quality=JPEG_QUALITY, stride=None):
+        """cv2.imencode('.jpg', img, [cv2.IMWRITE_JPEG_QUALITY, quality]) of a batch of BGR images on the device, byte for
+        byte (mocap_encode_jpeg_dev).  images: contiguous uint8 cuda tensor [..., H, W, 3], or with ``tiles`` > 1
+        [..., tiles, H, w, 3] -- each image is its ``tiles`` frames side by side (np.hstack), e.g. the frames of
+        ``live(..., want_frames=True)`` with tiles = C.  Returns {"jpeg": uint8 [n, stride], "len": int32 [n]} on the
+        device: image i is jpeg[i, :len[i]], len -1 where it did not fit ``stride`` (default: the worst case).  No
+        synchronisation."""
+        torch = _torch()
+        if images.dtype != torch.uint8 or not images.is_cuda or not images.is_contiguous() or images.dim() < 3 or images.shape[-1] != 3:
+            raise ValueError("encode_jpeg: images must be a contiguous uint8 cuda tensor [..., H, W, 3]")
+        tiles = int(tiles)
+        if tiles > 1 and (images.dim() < 4 or images.shape[-4] != tiles):
+            raise ValueError(f"encode_jpeg: with tiles={tiles} images must be [..., {tiles}, H, w, 3]")
+        th, tw = int(images.shape[-3]), int(images.shape[-2])
+        per = max(1, tiles) * th * tw * 3
+        n = images.numel() // per if per else 0
+        if stride is None:
+            stride = self.jpeg_bound(max(1, tiles) * tw, th)
+        jbuf = torch.empty((n, int(stride)), dtype=torch.uint8, device=images.device)
+        jlen = torch.empty((n,), dtype=torch.int32, device=images.device)
+        self.use_current_stream()
+        self._check(self.lib.mocap_encode_jpeg_dev(self.h, _ptr(images), n, tiles, tw, th, int(quality), _ptr(jbuf), int(stride), _ptr(jlen)))
+        return {"jpeg": jbuf, "len": jlen}
 
     def undistort_map(self, cam):
         m1 = np.empty((self.height, self.width, 2), dtype=np.int16)
@@ -1070,14 +1114,17 @@ def _live_cameras(cams, s, frames):
     return st
 
 
-def camera_read(cams, session=None, clock=time.time):
+def camera_read(cams, session=None, clock=time.time, jpeg=None):
     """Replacement of ``Cameras._camera_read(self)`` (helpers.py:68-135) on the device: ``cams.cameras.read()``, then
     one ``live_host`` call whose mode follows ``is_capturing_points`` / ``is_triangulating_points`` /
     ``is_locating_objects`` as the reference nests them, then the reference's emits and serial writes
     (:func:`live_read_events`).  Returns the processed frames -- with the centre dots while capturing -- in the container
     type the driver gave.  The context is built from ``camera_params`` and the first read's size; poses and the world
     matrix are re-sent only when their values change; a new ``kalman_filter`` object (start_trangulating_points) starts
-    a fresh device tracker, which reads ``clock`` once per read.  The filter object itself is never called."""
+    a fresh device tracker, which reads ``clock`` once per read.  The filter object itself is never called.
+    ``jpeg`` (a quality, 1..100): the same call also encodes the frames side by side on the device as
+    cv.imencode('.jpg', np.hstack(frames)) does at that quality (mocap_live_jpeg_host); returns (frames, the JPEG as
+    uint8 (N,))."""
     s = session or MocapSession.default()
     frames, _ = cams.cameras.read()
     capture = bool(cams.is_capturing_points)
@@ -1108,7 +1155,8 @@ def camera_read(cams, session=None, clock=time.time):
                 st.tracker, st.filter_obj = Tracker(ctx, int(cams.num_objects)), cams.kalman_filter
             tracker = st.tracker
         raw = np.stack([np.asarray(f, dtype=np.uint8) for f in frames])[None]
-        res = ctx.live_host(raw, mode, [float(clock())] if loc else None, tracker, want_frames=True)
+        res = ctx.live_host(raw, mode, [float(clock())] if loc else None, tracker, want_frames=True,
+                            **(dict(jpeg=True, quality=int(jpeg)) if jpeg is not None else {}))
     events, serial = live_read_events(res, 0, mode, cams.drone_armed if loc else ())
     for name, payload in events:
         cams.socketio.emit(name, payload)
@@ -1118,8 +1166,56 @@ def camera_read(cams, session=None, clock=time.time):
             time.sleep(0.001)
     out = res["frames"][0]
     if isinstance(frames, np.ndarray):
+        pass
+    elif isinstance(frames, tuple):
+        out = type(frames)(out[c] for c in range(len(out)))
+    else:
+        out = [out[c] for c in range(len(out))]
+    if jpeg is None:
         return out
-    return type(frames)(out[c] for c in range(len(out))) if isinstance(frames, tuple) else [out[c] for c in range(len(out))]
+    return out, res["jpeg"][0, :int(res["jpeg_len"][0])].copy()
+
+
+class StreamFrames(np.ndarray):
+    """What ``Cameras.get_frames`` returns under ``install_into(..., stream=True)``: np.hstack of the read's frames
+    (helpers.py:137-141), carrying the JPEG the device made of exactly these pixels -- ``jpeg`` uint8 (N,), made at
+    ``jpeg_quality`` -- for :class:`StreamCv`'s imencode.  It is read-only, so the bytes always describe its pixels; a
+    caller that draws on the frames draws on a copy (``np.array(frames)``), which carries nothing.  Views and results of
+    operations carry nothing either."""
+
+    def __array_finalize__(self, obj):
+        self.jpeg, self.jpeg_quality = None, None
+
+
+def stream_frames(frames, jpeg, quality):
+    out = np.hstack(list(frames)).view(StreamFrames)
+    out.jpeg, out.jpeg_quality = jpeg, int(quality)
+    out.flags.writeable = False
+    return out
+
+
+class StreamCv:
+    """A thin proxy of the cv2 module for the reference's index.py: ``imencode('.jpg' / '.jpeg', img, params)`` of a
+    :class:`StreamFrames` whose params ask for nothing but the quality its bytes were made at returns those bytes, as
+    ``(True, uint8 ndarray (N,))`` -- what cv2 returns for it, byte for byte.  Every other call and attribute is cv2's."""
+
+    def __init__(self, cv):
+        self.__dict__["_cv"] = cv
+
+    def __getattr__(self, name):
+        return getattr(self._cv, name)
+
+    def __setattr__(self, name, value):
+        setattr(self._cv, name, value)
+
+    def imencode(self, ext, img, params=None):
+        if isinstance(img, StreamFrames) and img.jpeg is not None and isinstance(ext, str) and ext.lower() in (".jpg", ".jpeg"):
+            p = [] if params is None else [int(v) for v in np.asarray(params).reshape(-1)]
+            pairs = list(zip(p[0::2], p[1::2]))
+            if len(p) % 2 == 0 and all(k == self._cv.IMWRITE_JPEG_QUALITY and v == img.jpeg_quality for k, v in pairs) \
+                    and (pairs or img.jpeg_quality == JPEG_QUALITY):
+                return True, img.jpeg.copy()
+        return self._cv.imencode(ext, img) if params is None else self._cv.imencode(ext, img, params)
 
 
 PATCHED_NAMES = ("triangulate_point", "triangulate_points", "calculate_reprojection_error",
@@ -1127,7 +1223,7 @@ PATCHED_NAMES = ("triangulate_point", "triangulate_points", "calculate_reproject
                  "bundle_adjustment", "locate_objects")
 
 
-def install_into(helpers_module, *also, session=None, tracker=False, large_holes=False, live=False):
+def install_into(helpers_module, *also, session=None, tracker=False, large_holes=False, live=False, stream=False):
     """Point a loaded reference ``helpers`` module at the CUDA path (INTEGRATION.md).
 
     ``also``: modules that imported the hot-path names BY VALUE -- the reference's ``index.py`` does
@@ -1147,7 +1243,15 @@ def install_into(helpers_module, *also, session=None, tracker=False, large_holes
 
     ``live=True`` also replaces ``_camera_read`` on the decorated class with :func:`camera_read`: the whole read --
     preprocessing, S1-S3, the world transform, locate_objects and the tracker -- in one device call per read, the
-    driver call, emits and serial writes staying in Python."""
+    driver call, emits and serial writes staying in Python.
+
+    ``stream=True`` (with ``live=True``) also moves the camera stream's JPEG encoding (index.py:55-56) into that call:
+    ``get_frames`` returns np.hstack of the read's frames as a :class:`StreamFrames` carrying the JPEG the device made of
+    them at cv2's default quality, and ``cv`` in every module of ``also`` that holds it is re-bound to a
+    :class:`StreamCv` proxy, whose ``imencode('.jpg', frames)`` returns those bytes -- cv2's, byte for byte -- and hands
+    every other call to cv2."""
+    if stream and not live:
+        raise ValueError("install_into: stream=True needs live=True (the JPEG is made in the live read's device call)")
     cams = helpers_module.Cameras.instance()
     s = session or MocapSession.install([np.asarray(p["intrinsic_matrix"], dtype=np.float64) for p in cams.camera_params],
                                         large_holes=large_holes)
@@ -1159,6 +1263,16 @@ def install_into(helpers_module, *also, session=None, tracker=False, large_holes
             return camera_read(self, s)
         _camera_read.__mocap_b200__ = True
         type(cams)._camera_read = _camera_read
+    if stream:
+        def get_frames(self):
+            frames, jpeg = camera_read(self, s, jpeg=JPEG_QUALITY)
+            return stream_frames(frames, jpeg, JPEG_QUALITY)
+        get_frames.__mocap_b200__ = True
+        type(cams).get_frames = get_frames
+        for mod in also:
+            cv = getattr(mod, "cv", None)
+            if cv is not None and not isinstance(cv, StreamCv):
+                mod.cv = StreamCv(cv)
     repl = {
         "triangulate_point": lambda ip, cp: triangulate_point(ip, cp, s),
         "triangulate_points": lambda ip, cp: triangulate_points(ip, cp, s),

@@ -194,6 +194,7 @@ void mocap_destroy(mocap_ctx* ctx) {
     cudaFree(ctx->d_live_in); cudaFree(ctx->d_live_out);
     if (ctx->h_live_in) cudaFreeHost(ctx->h_live_in);
     if (ctx->h_live_out) cudaFreeHost(ctx->h_live_out);
+    jpeg_release(ctx);
     cudaFree(ctx->d_stat_acc);
     if (ctx->h_stat) cudaFreeHost(const_cast<unsigned long long*>(ctx->h_stat));
     if (ctx->copy_stream) cudaStreamDestroy(ctx->copy_stream);

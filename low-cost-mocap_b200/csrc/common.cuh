@@ -79,6 +79,12 @@ struct mocap_ctx {
     // mocap_live_host staging: device and page-locked host buffers of {timestamps, raw frames} and {result, frames}
     uint8_t*  d_live_in; uint8_t* h_live_in; size_t live_in_bytes;
     uint8_t*  d_live_out; uint8_t* h_live_out; size_t live_out_bytes;
+    // JPEG encoder (jpeg.cu): device tables + header per (width, height, quality), scratch of a group of images, and
+    // mocap_live_jpeg_host's device output and page-locked staging
+    uint8_t*  jpeg_cfg[16]; int jpeg_cfg_key[16][3]; int jpeg_cfg_n;
+    uint8_t*  d_jpeg_scratch; size_t jpeg_scratch_bytes;
+    uint8_t*  d_jpeg_out; size_t jpeg_out_bytes;
+    uint8_t*  h_jpeg_out; size_t jpeg_host_bytes;
     // accounting
     uint64_t  launches;
     int       timing_on;
@@ -113,6 +119,25 @@ struct LiveOut {
     int mode;                   // MOCAP_LIVE_* bits
 };
 int launch_live_blobs(mocap_ctx* ctx, const LiveOut& live, int s0, int n_sets, int have_blobs, uint8_t* frames);
+// mocap_live_host in two halves (live.cu), so that mocap_live_jpeg_host runs the same chain: live_check; live_host_run
+// (staging in, the chain; the frames stay on the device when keep_frames); live_host_finish (result, frames and
+// extra_bytes of device data back, one synchronisation)
+struct LiveHostRun {
+    mocap_live_offsets L;
+    size_t res_bytes, frame_bytes, frame_copy, extra_bytes;
+    uint8_t* d_frames;
+};
+int live_check(mocap_ctx* ctx, mocap_tracker* tr, const void* raw, int n_reads, int mode, const double* timestamps,
+               const void* result, const char* who);
+int live_host_run(mocap_ctx* ctx, mocap_tracker* tr, const uint8_t* raw, int n_reads, int mode, const double* timestamps,
+                  int keep_frames, size_t extra_bytes, LiveHostRun* run);
+int live_host_finish(mocap_ctx* ctx, const LiveHostRun& run, uint8_t* frames, void* result, const void* extra, void* extra_out);
+// the JPEG encoder (jpeg.cu): mocap_encode_jpeg_dev after its checks; the context's JPEG buffers freed
+int jpeg_encode(mocap_ctx* ctx, const uint8_t* images, int n_images, int tiles, int tile_w, int tile_h, int quality,
+                uint8_t* out, uint64_t out_stride, int32_t* out_len);
+void jpeg_release(mocap_ctx* ctx);
+#define MOCAP_JPEG_CONFIGS 16                     // (width, height, quality) configurations cached per context
+#define JPEG_CONFIG_BYTES  3200                   // JpegTables + the header, padded (jpeg.cuh)
 // raw frames -> preprocessing [-> S1 [-> S2+S3]] per launch group (preproc.cu)
 enum { RAW_PREPROCESS = 0, RAW_DETECT = 1, RAW_MATCH = 2 };
 int run_raw_groups(mocap_ctx* ctx, const uint8_t* raw_frames, int n_frame_sets, int threshold, int stages, uint8_t* processed,

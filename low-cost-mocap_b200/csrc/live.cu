@@ -71,9 +71,9 @@ static void live_offsets(const mocap_config& c, int R, int D, mocap_live_offsets
     L->total = at;
 }
 
-// the checks both entry points make before anything is launched or copied
-static int live_check(mocap_ctx* ctx, mocap_tracker* tr, const void* raw, int n_reads, int mode, const double* timestamps,
-                      const void* result, const char* who) {
+// the checks the entry points make before anything is launched or copied
+int live_check(mocap_ctx* ctx, mocap_tracker* tr, const void* raw, int n_reads, int mode, const double* timestamps,
+               const void* result, const char* who) {
     if (!raw || !result || n_reads < 0) return mocap_fail(ctx, MOCAP_EINVAL, "%s: bad argument", who);
     if (mode != 0 && mode != LIVE_CAPTURE && mode != (LIVE_CAPTURE | LIVE_TRIANGULATE) &&
         mode != (LIVE_CAPTURE | LIVE_TRIANGULATE | LIVE_LOCATE))
@@ -154,30 +154,50 @@ int mocap_live_host(mocap_ctx* ctx, mocap_tracker* tr, const uint8_t* raw, int n
     if (!ctx) return MOCAP_EINVAL;
     int st = live_check(ctx, tr, raw, n_reads, mode, timestamps, result, "mocap_live_host");
     if (st || n_reads == 0) return st;
+    LiveHostRun run;
+    if ((st = live_host_run(ctx, tr, raw, n_reads, mode, timestamps, frames != nullptr, 0, &run)) != MOCAP_OK) return st;
+    return live_host_finish(ctx, run, frames, result, nullptr, nullptr);
+}
+
+}  // extern "C"
+
+// mocap_live_host up to the chain: staging in, live_run.  The processed frames stay on the device at run->d_frames when
+// keep_frames; extra_bytes more of page-locked staging are kept for live_host_finish.
+int live_host_run(mocap_ctx* ctx, mocap_tracker* tr, const uint8_t* raw, int n_reads, int mode, const double* timestamps,
+                  int keep_frames, size_t extra_bytes, LiveHostRun* run) {
+    int st;
     CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));
     const int C = ctx->cfg.n_cam, S = ctx->cfg.width;
-    mocap_live_offsets L;
+    mocap_live_offsets& L = run->L;
     live_offsets(ctx->cfg, n_reads, tr ? tracker_num_objects(tr) : 0, &L);
     const size_t ts_bytes = (mode & LIVE_LOCATE) ? (((size_t)n_reads * sizeof(double) + 255) & ~(size_t)255) : 0;
     const size_t raw_bytes = (size_t)n_reads * C * ctx->pp_in_w * ctx->pp_in_h * 3;
-    const size_t res_bytes = (L.total + 255) & ~(size_t)255;
-    const size_t frame_bytes = frames ? (size_t)n_reads * C * S * S * 3 : 0;
+    run->res_bytes = (L.total + 255) & ~(size_t)255;
+    run->frame_bytes = keep_frames ? (((size_t)n_reads * C * S * S * 3 + 255) & ~(size_t)255) : 0;
+    run->frame_copy = keep_frames ? (size_t)n_reads * C * S * S * 3 : 0;
+    run->extra_bytes = extra_bytes;
     if ((st = ensure_live_buffers(ctx, &ctx->d_live_in, &ctx->h_live_in, &ctx->live_in_bytes, ts_bytes + raw_bytes)) != MOCAP_OK) return st;
-    if ((st = ensure_live_buffers(ctx, &ctx->d_live_out, &ctx->h_live_out, &ctx->live_out_bytes, res_bytes + frame_bytes)) != MOCAP_OK) return st;
+    if ((st = ensure_live_buffers(ctx, &ctx->d_live_out, &ctx->h_live_out, &ctx->live_out_bytes,
+                                  run->res_bytes + run->frame_bytes + extra_bytes)) != MOCAP_OK) return st;
     // the staging buffers are free here: the previous call returned after its synchronisation
     if (ts_bytes) memcpy(ctx->h_live_in, timestamps, (size_t)n_reads * sizeof(double));
     memcpy(ctx->h_live_in + ts_bytes, raw, raw_bytes);
     CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_live_in, ctx->h_live_in, ts_bytes + raw_bytes, cudaMemcpyHostToDevice, ctx->stream));
-    uint8_t* d_frames = frames ? ctx->d_live_out + res_bytes : nullptr;
-    st = live_run(ctx, tr, ctx->d_live_in + ts_bytes, n_reads, mode, ts_bytes ? reinterpret_cast<const double*>(ctx->d_live_in) : nullptr,
-                  d_frames, ctx->d_live_out);
-    if (st) return st;
-    CUDA_TRY(ctx, cudaMemcpyAsync(ctx->h_live_out, ctx->d_live_out, L.total, cudaMemcpyDeviceToHost, ctx->stream));
-    if (frames) CUDA_TRY(ctx, cudaMemcpyAsync(ctx->h_live_out + res_bytes, d_frames, frame_bytes, cudaMemcpyDeviceToHost, ctx->stream));
-    CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-    memcpy(result, ctx->h_live_out, L.total);
-    if (frames) memcpy(frames, ctx->h_live_out + res_bytes, frame_bytes);
-    return MOCAP_OK;
+    run->d_frames = keep_frames ? ctx->d_live_out + run->res_bytes : nullptr;
+    return live_run(ctx, tr, ctx->d_live_in + ts_bytes, n_reads, mode, ts_bytes ? reinterpret_cast<const double*>(ctx->d_live_in) : nullptr,
+                    run->d_frames, ctx->d_live_out);
 }
 
-}  // extern "C"
+// the rest of mocap_live_host: the result, the frames (frames != NULL) and run.extra_bytes from the device pointer
+// `extra` back to the host, one synchronisation
+int live_host_finish(mocap_ctx* ctx, const LiveHostRun& run, uint8_t* frames, void* result, const void* extra, void* extra_out) {
+    uint8_t* h_extra = ctx->h_live_out + run.res_bytes + run.frame_bytes;
+    CUDA_TRY(ctx, cudaMemcpyAsync(ctx->h_live_out, ctx->d_live_out, run.L.total, cudaMemcpyDeviceToHost, ctx->stream));
+    if (frames) CUDA_TRY(ctx, cudaMemcpyAsync(ctx->h_live_out + run.res_bytes, run.d_frames, run.frame_copy, cudaMemcpyDeviceToHost, ctx->stream));
+    if (run.extra_bytes) CUDA_TRY(ctx, cudaMemcpyAsync(h_extra, extra, run.extra_bytes, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+    memcpy(result, ctx->h_live_out, run.L.total);
+    if (frames) memcpy(frames, ctx->h_live_out + run.res_bytes, run.frame_copy);
+    if (run.extra_bytes) memcpy(extra_out, h_extra, run.extra_bytes);
+    return MOCAP_OK;
+}
