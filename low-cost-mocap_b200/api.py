@@ -659,7 +659,7 @@ class MocapContext:
         self._check(self.lib.mocap_ba_residuals_host(self.h, _np_ptr(obs), _np_ptr(mask), F, _np_ptr(R), _np_ptr(t), _np_ptr(r), _np_ptr(valid), C.byref(nv)))
         return r[valid.astype(bool)]
 
-    def bundle_adjust(self, obs, mask, poses, ftol=1e-2, max_nfev=0, engine=0, prefit=True, jacobian=1):
+    def bundle_adjust(self, obs, mask, poses, ftol=1e-2, max_nfev=0, engine=0, prefit=True, jacobian=1, prefit_max_iter=50):
         obs = np.ascontiguousarray(obs, dtype=np.float64)
         mask = np.ascontiguousarray(mask, dtype=np.uint8)
         R = np.ascontiguousarray(np.stack([np.asarray(p["R"], dtype=np.float64).reshape(3, 3) for p in poses]))
@@ -668,7 +668,7 @@ class MocapContext:
         self.lib.mocap_ba_default_options(C.byref(opt))
         opt.ftol = ftol
         opt.max_nfev = max_nfev
-        opt.engine, opt.prefit, opt.jacobian = engine, 1 if prefit else 0, jacobian
+        opt.engine, opt.prefit, opt.jacobian, opt.prefit_max_iter = engine, 1 if prefit else 0, jacobian, prefit_max_iter
         rep = BAReport()
         self._check(self.lib.mocap_bundle_adjust_host(self.h, _np_ptr(obs), _np_ptr(mask), obs.shape[0], _np_ptr(R), _np_ptr(t), C.byref(opt), C.byref(rep)))
         out = [{"R": R[i].copy(), "t": t[i].copy()} for i in range(R.shape[0])]

@@ -495,8 +495,8 @@ void exp_so3(const double w[3], double E[9]) {
     for (int i = 0; i < 9; ++i) E[i] = (i % 4 == 0 ? 1.0 : 0.0) + a * K[i] + b * K2[i];
 }
 
-// Levenberg-Marquardt over poses + points.  Rt: [C][12] in/out.
-int prefit(DeviceBA& P, std::vector<double>& Rt, int max_iter, mocap_ba_report* rep) {
+// Levenberg-Marquardt over poses + points.  Rt: [C][12] in/out; *taken: whether a step was accepted.
+int prefit(DeviceBA& P, std::vector<double>& Rt, int max_iter, mocap_ba_report* rep, bool* taken) {
     mocap_ctx* ctx = P.ctx;
     cudaStream_t s = ctx->stream;
     const int C = P.C, m = P.m, n = 6 * (C - 1);
@@ -522,6 +522,7 @@ int prefit(DeviceBA& P, std::vector<double>& Rt, int max_iter, mocap_ba_report* 
     int st = eval_cost(P.d_X, &cost);
     if (st) return st;
     rep->prefit_cost_initial = cost;
+    *taken = false;
     int it = 0;
     for (; it < max_iter; ++it) {
         CUDA_TRY(ctx, cudaMemsetAsync(P.d_sba, 0, n_out * sizeof(double), s));
@@ -533,7 +534,13 @@ int prefit(DeviceBA& P, std::vector<double>& Rt, int max_iter, mocap_ba_report* 
         S.assign(out.begin(), out.begin() + (size_t)n * n);
         rhs.assign(n, 0.0);
         for (int i = 0; i < n; ++i) { S[(size_t)i * n + i] += lambda * out[(size_t)n * n + n + i]; rhs[i] = -out[(size_t)n * n + i]; }
-        if (!cholesky_solve(n, S, rhs)) { lambda *= 10.0; if (lambda > 1e12) break; continue; }
+        // a parameter with a zero diagonal belongs to a camera that sees no point: pinned, its step is 0 (ba_device.cuh)
+        for (int i = 0; i < n; ++i)
+            if (out[(size_t)n * n + n + i] == 0.0) {
+                for (int j = 0; j < n; ++j) S[(size_t)i * n + j] = S[(size_t)j * n + i] = 0.0;
+                S[(size_t)i * n + i] = 1.0; rhs[i] = 0.0;
+            }
+        if (!cholesky_solve(n, S, rhs)) { lambda *= 10.0; if (lambda > 1e12) { ++it; break; } continue; }
         // candidate poses: R' = Exp(dw) R, t' = t + dt
         Rt_new = Rt;
         for (int c = 1; c < C; ++c) {
@@ -562,13 +569,14 @@ int prefit(DeviceBA& P, std::vector<double>& Rt, int max_iter, mocap_ba_report* 
             Rt = Rt_new;
             double* tmp = P.d_X; P.d_X = P.d_Xnew; P.d_Xnew = tmp;
             cost = cost_new;
+            *taken = true;
             lambda = fmax(lambda * 0.3, 1e-12);
             if (rel < BA_PREFIT_REL_STOP) { ++it; break; }
         } else {
             CUDA_TRY(ctx, upload(Rt));                       // back to the accepted poses
             CUDA_TRY(ctx, cudaStreamSynchronize(s));
             lambda *= 10.0;
-            if (lambda > 1e12) break;
+            if (lambda > 1e12) { ++it; break; }
         }
     }
     CUDA_TRY(ctx, upload(Rt));
@@ -723,13 +731,14 @@ int mocap_bundle_adjust_host(mocap_ctx* ctx, const double* obs, const uint8_t* m
     std::vector<double> x;
     x_from_poses(ctx, R, t, C, x);                              // helpers.py:278-285
 
+    bool taken = false;
     if (opt.prefit) {
         // start from the DLT points of the initial poses (k_ba_eval writes them to d_X)
         st = P.eval(x.data(), false);
         if (st) return st;
         std::vector<double> Rt;
         DeviceBA::poses_from_x(x.data(), C, Rt);
-        st = prefit(P, Rt, opt.prefit_max_iter > 0 ? opt.prefit_max_iter : 50, &rep);
+        st = prefit(P, Rt, opt.prefit_max_iter > 0 ? opt.prefit_max_iter : 50, &rep, &taken);
         if (st) return st;
         for (int c = 1; c < C; ++c) {
             double Rc[9];
@@ -740,9 +749,10 @@ int mocap_bundle_adjust_host(mocap_ctx* ctx, const double* obs, const uint8_t* m
         }
     }
 
-    // after the prefit the start is already close: begin the polish with a trust region of 0.01 (rad / pose
-    // units) instead of scipy's ||x0|| (~ the focal length), which would burn its evaluations shrinking
-    trf::Options topt{opt.ftol, opt.xtol, opt.gtol, opt.max_nfev, opt.prefit ? BA_POLISH_RADIUS : 0.0};
+    // after a prefit that took a step the start is already close: begin the polish with a trust region of
+    // BA_POLISH_RADIUS (rad / pose units) instead of scipy's ||x0|| (~ the focal length), which would burn its evaluations
+    // shrinking.  A prefit that took no step left the start where it was: the polish starts as scipy does
+    trf::Options topt{opt.ftol, opt.xtol, opt.gtol, opt.max_nfev, taken ? BA_POLISH_RADIUS : 0.0};
     trf::Report trep{};
     st = trf::minimize(P, x.data(), topt, trep);
     if (st) return st;

@@ -35,7 +35,7 @@
 // host-stepped solve in ba.cu): the polish that follows works on a float32-quantised objective whose resolution is
 // coarser than that
 #define BA_PREFIT_REL_STOP 1e-7
-// trust radius the polish starts with after a prefit (rad / pose units; scipy would start at ||x0|| ~ the focal length and
+// trust radius the polish starts with after a prefit that took a step (rad / pose units; scipy would start at ||x0|| ~ the focal length and
 // spend its evaluations shrinking).  The prefit ends within ~1e-5 of the reference objective's own minimiser, and scipy's
 // radius doubles whenever a step at the boundary is good, so a small start costs nothing when more room is needed;
 // measured on the three S4 goldens: 1e-2 -> 7 evaluations, 1e-4 -> 4, final costs equal to 1e-4 relative (the float32
@@ -344,7 +344,7 @@ struct BACtrl {
     double cost, cost_new, cost_initial, Delta, alpha, lambda, g_norm, pred, step_norm, actual, pcost, pcost_new;
     double pf_cost0, pf_cost1;
     double tr_alpha, tr_lower, tr_upper, tr_conv, a_diag, hh_beta, hh_alpha, hh_K;
-    int m, ntiles, n_valid, nfev, njev, iteration, termination, finite, flag, go, pf_it, accepted, tr_its, tr_calls;
+    int m, ntiles, n_valid, nfev, njev, iteration, termination, finite, flag, go, pf_it, pf_taken, accepted, tr_its, tr_calls;
     int cta, ncta;                     // this CTA's index in its problem's sub-grid, and the sub-grid's size
 };
 
@@ -1140,7 +1140,7 @@ BA_DEV void ba_solve_body(const BAParams& P, const BAParams& Q, unsigned char* s
     ba_grid_sum3(P, S, slot, v3, tot); slot ^= 1;
     if (tid == 0) {
         ctl->cost_initial = tot[0]; ctl->cost = tot[0]; ctl->finite = tot[1] == 0.0; ctl->n_valid = (int)tot[2];
-        ctl->pf_cost0 = 0.0; ctl->pf_cost1 = 0.0; ctl->pf_it = 0;
+        ctl->pf_cost0 = 0.0; ctl->pf_cost1 = 0.0; ctl->pf_it = 0; ctl->pf_taken = 0;
         ctl->nfev = 0; ctl->njev = 0; ctl->iteration = 0; ctl->termination = -99; ctl->g_norm = 0.0; ctl->tr_its = 0; ctl->tr_calls = 0;
     }
     __syncthreads();
@@ -1172,13 +1172,16 @@ BA_DEV void ba_solve_body(const BAParams& P, const BAParams& Q, unsigned char* s
             BA_TICK(BA_PH_PF_SYSTEM);
             if (tid == 0) {
                 const double c0 = ba_fresh(P.fin)[npair + 2 * n];
-                if (ctl->pcost < 0.0) ctl->pf_cost0 = c0;
+                if (ctl->pcost < 0.0) { ctl->pf_cost0 = c0; ctl->pf_cost1 = c0; }
                 ctl->pcost = c0;
                 ctl->flag = 1;
             }
+            // a parameter with a zero diagonal belongs to a camera that sees no point: its rows of the reduced system are
+            // zero at every lambda, so it is pinned (unit diagonal, zero right-hand side) and its step is 0
             for (int e = tid; e < n * n; e += nt) {
                 const int i = e / n, j = e - i * n;
-                S.L[e] = S.A[e] + (i == j ? lambda * ba_fresh(P.fin)[npair + n + i] : 0.0);
+                const double Di = ba_fresh(P.fin)[npair + n + i], Dj = ba_fresh(P.fin)[npair + n + j];
+                S.L[e] = (Di == 0.0 || Dj == 0.0) ? (i == j ? 1.0 : 0.0) : S.A[e] + (i == j ? lambda * Di : 0.0);
             }
             __syncthreads();
             const bool pd = ba_chol_factor(S.L, n, &ctl->flag);
@@ -1189,7 +1192,7 @@ BA_DEV void ba_solve_body(const BAParams& P, const BAParams& Q, unsigned char* s
                 __syncthreads();
                 continue;
             }
-            for (int i = tid; i < n; i += nt) S.p[i] = -S.g[i];
+            for (int i = tid; i < n; i += nt) S.p[i] = ba_fresh(P.fin)[npair + n + i] == 0.0 ? 0.0 : -S.g[i];
             __syncthreads();
             ba_solve_lower(S.L, n, S.p);
             ba_solve_upper(S.L, n, S.p);                           // dc
@@ -1231,6 +1234,7 @@ BA_DEV void ba_solve_body(const BAParams& P, const BAParams& Q, unsigned char* s
                 if (tid == 0) {
                     const double rel = (cost - cost_new) / fmax(cost, 1e-300);
                     ctl->pf_cost1 = cost_new;
+                    ctl->pf_taken = 1;
                     ctl->lambda = fmax(lambda * 0.3, 1e-12);
                     if (rel < BA_PREFIT_REL_STOP) ctl->go = 0;
                 }
@@ -1270,7 +1274,8 @@ BA_DEV void ba_solve_body(const BAParams& P, const BAParams& Q, unsigned char* s
         ctl->cost = ba_fresh(P.fin)[npair + n]; ctl->finite = ba_fresh(P.fin)[npair + n + 1] == 0.0;
         if (!Q.prefit) ctl->cost_initial = ctl->cost;
         ctl->nfev = 1; ctl->njev = 1;
-        double D = Q.prefit ? BA_POLISH_RADIUS : ba_norm2_serial(S.x, nf);     // after the prefit the start is already close (ba.cu)
+        // after a prefit that took a step the start is already close (ba.cu); otherwise the polish starts as scipy does
+        double D = (Q.prefit && ctl->pf_taken) ? BA_POLISH_RADIUS : ba_norm2_serial(S.x, nf);
         if (D == 0.0) D = 1.0;
         ctl->Delta = D; ctl->alpha = 0.0; ctl->iteration = 0; ctl->termination = -99;
         if (!ctl->finite) ctl->termination = -1;
