@@ -297,15 +297,14 @@ def test_preprocess_tile_stages_fuzz_on_host(preproc_host):
     coordinates far outside the frame), both rotations, several thread counts."""
     import cv2
     from oracle.ref_port import RefPort
+    from tests.preproc_util import fuzz_camera
     rng = np.random.default_rng(2024)
     p = lambda a: a.ctypes.data_as(ctypes.c_void_p) if a is not None else None
     for case in range(24):
         S = int(rng.integers(34, 150))
         in_h = int(rng.integers(1, S - 15)) if case % 4 else S - 16
         rot = int(rng.choice([0, 2]))
-        f0 = float(rng.uniform(0.5, 1.5) * S)
-        K = np.array([[f0, 0, S / 2.0 + rng.uniform(-5, 5)], [0, f0 * rng.uniform(0.9, 1.1), S / 2.0 + rng.uniform(-5, 5)], [0, 0, 1]])
-        dist = np.array([-0.126, 0.263, 0.0012, 0.0002, -0.249]) * rng.uniform(-3.0, 3.0)
+        K, dist = fuzz_camera(rng, S)
         m1, m2 = cv2.initUndistortRectifyMap(K, dist, np.eye(3), K, (S, S), cv2.CV_16SC2)
         m1 = np.ascontiguousarray(m1); m2 = np.ascontiguousarray(m2)
         raw = rng.integers(0, 256, size=(2, in_h, S, 3), dtype=np.uint8)
