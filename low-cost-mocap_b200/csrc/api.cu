@@ -10,7 +10,6 @@
 int blob_kernels_init(mocap_ctx* ctx);
 int match_kernels_init(mocap_ctx* ctx);
 int fused_kernel_init(mocap_ctx* ctx);
-int tma_kernel_init(mocap_ctx* ctx);
 int ba_dev_init(mocap_ctx* ctx);
 
 int mocap_fail(mocap_ctx* ctx, int code, const char* fmt, ...) {
@@ -146,12 +145,10 @@ int mocap_create(mocap_ctx** out, const mocap_config* cfg) {
         if ((st = blob_kernels_init(ctx)) != MOCAP_OK) break;
         if ((st = match_kernels_init(ctx)) != MOCAP_OK) break;
         {
-            // MOCAP_PIPELINE = split | fused | phased | tma pins the pipeline (A/B measurements); unset: single-pass kernel,
+            // MOCAP_PIPELINE = split | fused pins the pipeline (A/B measurements); unset: single-pass kernel,
             // except for batches of heavy frame-sets (see pick_fused)
             const char* mode = getenv("MOCAP_PIPELINE");
             ctx->use_fused = (mode && strcmp(mode, "split") == 0) ? 0 : 1;
-            ctx->use_tma = (mode && strcmp(mode, "tma") == 0) ? 1 : 0;
-            ctx->use_phased = (mode && strcmp(mode, "phased") == 0) ? 1 : 0;
             ctx->pipeline_auto = (mode && mode[0]) ? 0 : 1;
         }
         {
@@ -166,9 +163,7 @@ int mocap_create(mocap_ctx** out, const mocap_config* cfg) {
             if (cudaMemset(ctx->d_stat_acc, 0, sizeof(unsigned long long)) != cudaSuccess) { st = MOCAP_ECUDA; break; }
         }
         if ((st = fused_kernel_init(ctx)) != MOCAP_OK) break;
-        if ((st = tma_kernel_init(ctx)) != MOCAP_OK) break;
         if ((st = ba_dev_init(ctx)) != MOCAP_OK) break;
-        if (ctx->tma_ctas_per_sm < 1) ctx->use_tma = 0;
     } while (0);
     if (st != MOCAP_OK) { mocap_destroy(ctx); return st; }
     *out = ctx;
@@ -247,9 +242,8 @@ int mocap_set_world_transform(mocap_ctx* ctx, const double* M) {
 // batch take the three-kernel pipeline.  The blob count of the previous batch arrives through mapped host memory
 // (written by the last CTA of the blob fallback kernel): no synchronisation, a stale or torn value only steers
 // this heuristic, both pipelines give the same results.
-static bool pick_fused(const mocap_ctx* ctx, int channels) {
+static bool pick_fused(const mocap_ctx* ctx) {
     if (!ctx->use_fused) return false;
-    if (channels != 1 && (ctx->use_tma || ctx->use_phased)) return false;     // the experimental variants stream 1-channel frames only
     if (!ctx->pipeline_auto) return true;
     const unsigned long long blobs = ctx->h_stat[0], images = ctx->h_stat[1];
     if (images == 0) return true;
@@ -296,7 +290,7 @@ int mocap_pipeline_tracks_dev(mocap_ctx* ctx, const uint8_t* frames, int n_frame
     CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));
     const int C = ctx->cfg.n_cam;
     const size_t set_bytes = (size_t)C * ctx->cfg.width * ctx->cfg.height * channels;
-    const bool fused = pick_fused(ctx, channels);
+    const bool fused = pick_fused(ctx);
     // frame-sets per launch group: bounds the segment-list scratch (max_segments * 4 B per image)
     const int chunk = fused ? (65536 / C > 0 ? 65536 / C : 1) : 4096;
     int st = ensure_images(ctx, (n_frame_sets < chunk ? n_frame_sets : chunk) * C);
@@ -306,12 +300,8 @@ int mocap_pipeline_tracks_dev(mocap_ctx* ctx, const uint8_t* frames, int n_frame
         // the launchers hand this to the matcher (frame-set indices inside a launch group start at 0)
         ctx->track_xy_cur = track_xy ? track_xy + (size_t)s0 * ctx->cfg.max_roots * C * 2 : nullptr;
         if (fused) {
-            if (ctx->use_tma)
-                st = launch_pipeline_tma(ctx, frames + (size_t)s0 * set_bytes, ns, threshold, obj + (size_t)s0 * ctx->cfg.max_roots * 3,
-                                         err + (size_t)s0 * ctx->cfg.max_roots, n_obj + s0, set_flags ? set_flags + s0 : nullptr);
-            else
-                st = launch_pipeline_fused(ctx, frames + (size_t)s0 * set_bytes, ns, threshold, obj + (size_t)s0 * ctx->cfg.max_roots * 3,
-                                           err + (size_t)s0 * ctx->cfg.max_roots, n_obj + s0, set_flags ? set_flags + s0 : nullptr, channels);
+            st = launch_pipeline_fused(ctx, frames + (size_t)s0 * set_bytes, ns, threshold, obj + (size_t)s0 * ctx->cfg.max_roots * 3,
+                                       err + (size_t)s0 * ctx->cfg.max_roots, n_obj + s0, set_flags ? set_flags + s0 : nullptr, channels);
             if (st) break;
             continue;
         }
@@ -357,7 +347,7 @@ int mocap_pipeline_host(mocap_ctx* ctx, const uint8_t* frames, int n_frame_sets,
     CUDA_TRY(ctx, cudaEventRecord(copied[0], ctx->stream));
     CUDA_TRY(ctx, cudaStreamWaitEvent(ctx->copy_stream, copied[0], 0));
     CUDA_TRY(ctx, cudaStreamWaitEvent(ctx->copy_stream2, copied[0], 0));
-    const bool fused = pick_fused(ctx, channels);
+    const bool fused = pick_fused(ctx);
     int k = 0, n_chunks = 0;
     for (int s0 = 0; s0 < n_frame_sets; s0 += chunk, k ^= 1, ++n_chunks) {
         const int ns = (n_frame_sets - s0 < chunk) ? n_frame_sets - s0 : chunk;
@@ -368,12 +358,8 @@ int mocap_pipeline_host(mocap_ctx* ctx, const uint8_t* frames, int n_frame_sets,
         CUDA_TRY(ctx, cudaEventRecord(copied[k], cs));
         CUDA_TRY(ctx, cudaStreamWaitEvent(ctx->stream, copied[k], 0));
         if (fused) {
-            if (ctx->use_tma)
-                st = launch_pipeline_tma(ctx, ctx->d_stage[k], ns, threshold, ctx->d_obj + (size_t)s0 * RM * 3, ctx->d_err + (size_t)s0 * RM,
-                                         ctx->d_nobj + s0, ctx->d_setflags + s0);
-            else
-                st = launch_pipeline_fused(ctx, ctx->d_stage[k], ns, threshold, ctx->d_obj + (size_t)s0 * RM * 3, ctx->d_err + (size_t)s0 * RM,
-                                           ctx->d_nobj + s0, ctx->d_setflags + s0, channels);
+            st = launch_pipeline_fused(ctx, ctx->d_stage[k], ns, threshold, ctx->d_obj + (size_t)s0 * RM * 3, ctx->d_err + (size_t)s0 * RM,
+                                       ctx->d_nobj + s0, ctx->d_setflags + s0, channels);
             if (st) break;
             CUDA_TRY(ctx, cudaEventRecord(ctx->stage_free[k], ctx->stream));
             continue;

@@ -46,9 +46,6 @@ struct mocap_ctx {
     uint32_t* d_set_done;     // fused kernel: [2*cap_images] finished images per set, then deferred marks
     unsigned long long* d_unit_counter;
     int       fused_ctas_per_sm;
-    int       tma_ctas_per_sm;   // 0: bulk-copy kernel unavailable for this configuration
-    int       use_tma;           // MOCAP_PIPELINE=tma: stream through the bulk-copy ring kernel
-    int       use_phased;        // MOCAP_PIPELINE=phased: phase-synchronous variant of the single-pass kernel (opt-in, fused_phased.cuh)
     int       pipeline_auto;     // MOCAP_PIPELINE unset: heavy batches (many blobs per frame-set) take the three-kernel pipeline
     unsigned long long* d_stat_acc;                  // device accumulator of the blob statistic
     volatile unsigned long long* h_stat;             // pinned, mapped: {blobs, images} of the last batch, written by the GPU
@@ -156,8 +153,6 @@ int blob_set_large_holes(mocap_ctx* ctx, int on);
 #define MOCAP_MATCH_CHUNK 512
 int launch_match_list(mocap_ctx* ctx, const int32_t* blob_xy, const int32_t* blob_n, const uint32_t* set_list, uint32_t* set_count,
                       int n_sets_max, double* obj, double* err, int32_t* n_obj, int32_t* set_flags);
-int launch_pipeline_tma(mocap_ctx* ctx, const uint8_t* frames, int n_sets, int threshold,
-                        double* obj, double* err, int32_t* n_obj, int32_t* set_flags);
 int launch_pipeline_fused(mocap_ctx* ctx, const uint8_t* frames, int n_sets, int threshold,
                           double* obj, double* err, int32_t* n_obj, int32_t* set_flags, int channels = 1);
 int timing_flush(mocap_ctx* ctx);

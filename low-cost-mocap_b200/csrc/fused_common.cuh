@@ -1,5 +1,5 @@
-// Pieces shared by the two single-pass pipeline kernels (fused_kernel.cu: plain streaming loads;
-// tma_kernel.cu: bulk-copy ring): parameters and the "last arriver" follow-up work.
+// Pieces of the single-pass pipeline kernel (fused_device.cuh, launched by fused_kernel.cu): its parameters and
+// the "last arriver" follow-up work.
 #pragma once
 #include "common.cuh"
 #include "blob_device.cuh"

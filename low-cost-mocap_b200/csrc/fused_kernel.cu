@@ -14,7 +14,6 @@
 // separate kernels after it.  Images / frame-sets beyond the warp-level capacities are put on
 // worklists and finished by the full-size kernels (k_blob_reduce, k_match_triangulate) afterwards.
 #include "fused_device.cuh"
-#include "fused_phased.cuh"
 
 size_t fused_slab_bytes(const mocap_config& c) {
     size_t a = sizeof(WarpSlab), b = warp_state_bytes(c.max_roots, c.n_cam, c.max_cands, c.max_blobs);
@@ -56,7 +55,7 @@ int launch_pipeline_fused(mocap_ctx* ctx, const uint8_t* frames, int n_sets, int
     P.obj = obj; P.err = err; P.n_obj = n_obj; P.set_flags = set_flags;
     P.track_xy = ctx->track_xy_cur;
     P.slab_bytes = fused_slab_bytes(c);
-    const size_t smem = P.slab_bytes * FUSED_WARPS + (ctx->use_phased ? sizeof(PhasedQueues) : 0);
+    const size_t smem = P.slab_bytes * FUSED_WARPS;
     const long long mx = c.width > c.height ? c.width : c.height;
     const bool wide = 6ll * mx * c.width * c.height >= (1ll << 32);
 
@@ -66,15 +65,7 @@ int launch_pipeline_fused(mocap_ctx* ctx, const uint8_t* frames, int n_sets, int
         CUDA_TRY(ctx, cudaEventRecord(ctx->tim_ev[2 * ctx->tim_used], ctx->stream));
     }
     const int grid = ctx->num_sms * ctx->fused_ctas_per_sm;
-    if (ctx->use_phased) {                                   // MOCAP_PIPELINE=phased: phase-synchronous variant (fused_phased.cuh)
-        if (wide) {
-            if (P.tc.use_and) k_pipeline_phased<true, true><<<grid, FUSED_WARPS * 32, smem, ctx->stream>>>(P);
-            else k_pipeline_phased<true, false><<<grid, FUSED_WARPS * 32, smem, ctx->stream>>>(P);
-        } else {
-            if (P.tc.use_and) k_pipeline_phased<false, true><<<grid, FUSED_WARPS * 32, smem, ctx->stream>>>(P);
-            else k_pipeline_phased<false, false><<<grid, FUSED_WARPS * 32, smem, ctx->stream>>>(P);
-        }
-    } else if (channels == 3) {                             // H x W x 3 interleaved: the layout _find_dot receives
+    if (channels == 3) {                                     // H x W x 3 interleaved: the layout _find_dot receives
         if (wide) {
             if (P.tc.use_and) k_pipeline_fused<true, true, true><<<grid, FUSED_WARPS * 32, smem, ctx->stream>>>(P);
             else k_pipeline_fused<true, false, true><<<grid, FUSED_WARPS * 32, smem, ctx->stream>>>(P);
@@ -117,17 +108,7 @@ int fused_kernel_init(mocap_ctx* ctx) {
     CUDA_TRY(ctx, cudaFuncSetAttribute(k_pipeline_fused<false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     CUDA_TRY(ctx, cudaFuncSetAttribute(k_pipeline_fused<false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int per_sm = 0;      // persistent grid = what is actually co-resident
-    if (ctx->use_phased) {
-        const int psmem = (int)(smem + sizeof(PhasedQueues));
-        CUDA_TRY(ctx, cudaFuncSetAttribute(k_pipeline_phased<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, psmem));
-        CUDA_TRY(ctx, cudaFuncSetAttribute(k_pipeline_phased<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, psmem));
-        CUDA_TRY(ctx, cudaFuncSetAttribute(k_pipeline_phased<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, psmem));
-        CUDA_TRY(ctx, cudaFuncSetAttribute(k_pipeline_phased<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, psmem));
-        CUDA_TRY(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_pipeline_phased<false, false>, FUSED_WARPS * 32, psmem));
-        if (per_sm < 1) { ctx->use_phased = 0; per_sm = 0; }
-    }
-    if (!ctx->use_phased)
-        CUDA_TRY(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_pipeline_fused<false, false>, FUSED_WARPS * 32, smem));
+    CUDA_TRY(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_pipeline_fused<false, false>, FUSED_WARPS * 32, smem));
     if (per_sm < 1) { ctx->use_fused = 0; return MOCAP_OK; }
     ctx->fused_ctas_per_sm = per_sm;
     return MOCAP_OK;

@@ -6,7 +6,6 @@
 // NOT part of libmocap_b200.so and never used by the product path.
 #include "simt_emu.h"
 #include "../../low-cost-mocap_b200/csrc/fused_device.cuh"
-#include "../../low-cost-mocap_b200/csrc/fused_phased.cuh"
 #include "../../low-cost-mocap_b200/csrc/camera_tables.h"
 
 alignas(16) unsigned char smem_raw[64 * 1024 * 4];            // the kernel's `extern __shared__` array (one CTA)
@@ -14,9 +13,8 @@ alignas(16) unsigned char smem_raw[64 * 1024 * 4];            // the kernel's `e
 // frames uint8 [n_sets][C][H][W] -> obj [n_sets][RMAX][3], err [n_sets][RMAX], n_obj, set_flags, blob_xy
 // [n_img][MB][2], blob_n [n_img]; counters[0..1] = images / frame-sets left on the worklists, counters[2] = number of
 // self-resetting scratch words found non-zero after the run (must be 0), counters[3] = units claimed.
-// phased != 0: the phase-synchronous variant k_pipeline_phased (csrc/fused_phased.cuh) instead.
 extern "C" int hc_pipeline_fused(const uint8_t* frames, int n_sets, int C, int W, int H, int threshold, const double* K, const double* R,
-                                 const double* t, int MB, int E, int RMAX, int KC, unsigned GMAX, int n_warps, int runs, int phased,
+                                 const double* t, int MB, int E, int RMAX, int KC, unsigned GMAX, int n_warps, int runs,
                                  double* obj, double* err, int32_t* n_obj, int32_t* set_flags, int32_t* blob_xy, int32_t* blob_n,
                                  uint32_t* img_worklist, uint32_t* set_worklist, long long* counters, int channels) {
     static CameraTables T;
@@ -57,18 +55,14 @@ extern "C" int hc_pipeline_fused(const uint8_t* frames, int n_sets, int C, int W
     P.obj = obj; P.err = err; P.n_obj = n_obj; P.set_flags = set_flags;
     const size_t a = sizeof(WarpSlab), b = warp_state_bytes(RMAX, C, KC, MB);
     P.slab_bytes = ((a > b ? a : b) + 15) & ~(size_t)15;
-    if (phased) n_warps = FUSED_WARPS;                       // the phased kernel's loops are written for exactly this many warps
-    if (P.slab_bytes * n_warps + sizeof(PhasedQueues) > sizeof(smem_raw)) return -1;
+    if (P.slab_bytes * n_warps > sizeof(smem_raw)) return -1;
     const long long mx = W > H ? W : H;
     const bool wide = 6ll * mx * W * H >= (1ll << 32);
     for (int run = 0; run < runs; ++run) {                   // a second run must find every counter re-armed
         unit_counter = 0;                                    // (the launcher resets this one with a memset)
         if (run > 0 && (work_count[0] || work_count[2])) break;       // worklists are consumed by the fallback kernels
         simt::launch(32 * n_warps, [&] {
-            if (phased) {
-                if (wide) { if (P.tc.use_and) k_pipeline_phased<true, true>(P); else k_pipeline_phased<true, false>(P); }
-                else      { if (P.tc.use_and) k_pipeline_phased<false, true>(P); else k_pipeline_phased<false, false>(P); }
-            } else if (channels == 3) {
+            if (channels == 3) {
                 if (wide) { if (P.tc.use_and) k_pipeline_fused<true, true, true>(P); else k_pipeline_fused<true, false, true>(P); }
                 else      { if (P.tc.use_and) k_pipeline_fused<false, true, true>(P); else k_pipeline_fused<false, false, true>(P); }
             } else {

@@ -14,7 +14,6 @@ p = lambda a: a.ctypes.data_as(ctypes.c_void_p)
 z = load_golden(case, n=4)
 C, B = int(z["C"]), 4
 frames = np.ascontiguousarray(z["frames"][:B])
-phased = 1 if "phased" in sys.argv[4:] else 0
 if "crowded" in sys.argv[4:]:                            # a crowded image: the deferral path
     for k in range(70):
         y, x = 10 + 6 * (k // 35), 20 + 16 * (k % 35)
@@ -24,6 +23,6 @@ RM, MB, E = 128, 64, 1024
 obj = np.zeros((B, RM, 3)); err = np.zeros((B, RM)); k = np.zeros(B, np.int32); fl = np.zeros(B, np.int32)
 bxy = np.zeros((B * C, MB, 2), np.int32); bn = np.zeros(B * C, np.int32)
 iw = np.zeros(B * C, np.uint32); sw = np.zeros(B, np.uint32); cnt = np.zeros(4, np.int64)
-rc = lib.hc_pipeline_fused(p(frames), B, C, 640, 480, 51, p(K), p(R), p(t), MB, E, RM, 8, ctypes.c_uint(4096), 8, 2, phased,
-                           p(obj), p(err), p(k), p(fl), p(bxy), p(bn), p(iw), p(sw), p(cnt))
+rc = lib.hc_pipeline_fused(p(frames), B, C, 640, 480, 51, p(K), p(R), p(t), MB, E, RM, 8, ctypes.c_uint(4096), 8, 2,
+                           p(obj), p(err), p(k), p(fl), p(bxy), p(bn), p(iw), p(sw), p(cnt), 1)
 print("RESULT", rc, cnt.tolist(), k.tolist())

@@ -274,7 +274,7 @@ def fused_emu():
                            "-fno-strict-aliasing", "-o", out, src])
     lib = ctypes.CDLL(out)
 
-    def run(frames, K, R, t, threshold=51, max_blobs=64, E=1024, max_roots=128, max_cands=8, max_groups=4096, n_warps=8, runs=2, phased=0):
+    def run(frames, K, R, t, threshold=51, max_blobs=64, E=1024, max_roots=128, max_cands=8, max_groups=4096, n_warps=8, runs=2):
         frames = np.ascontiguousarray(frames, dtype=np.uint8)
         channels = 3 if frames.ndim == 5 else 1                 # [B, C, H, W, 3]: the interleaved layout _find_dot receives
         B, C, H, W = frames.shape[:4]
@@ -285,7 +285,7 @@ def fused_emu():
         iw = np.zeros(B * C, np.uint32); sw = np.zeros(B, np.uint32); cnt = np.zeros(4, np.int64)
         p = lambda a: a.ctypes.data_as(ctypes.c_void_p)
         rc = lib.hc_pipeline_fused(p(frames), B, C, W, H, int(threshold), p(K), p(R), p(t), max_blobs, E, max_roots, max_cands,
-                                   ctypes.c_uint(max_groups), n_warps, runs, phased, p(obj), p(err), p(k), p(fl), p(bxy), p(bn), p(iw), p(sw), p(cnt), channels)
+                                   ctypes.c_uint(max_groups), n_warps, runs, p(obj), p(err), p(k), p(fl), p(bxy), p(bn), p(iw), p(sw), p(cnt), channels)
         assert rc == 0
         return {"obj": obj, "err": err, "n": k, "flags": fl, "blob_xy": bxy.reshape(B, C, max_blobs, 2), "blob_n": bn.reshape(B, C),
                 "deferred_images": iw[:cnt[0]].tolist(), "deferred_sets": sw[:cnt[1]].tolist(), "dirty_scratch": int(cnt[2])}
@@ -383,7 +383,7 @@ def test_device_code_has_no_unintended_data_races(tmp_path):
     supp = tmp_path / "supp.txt"
     supp.write_text("race:uf_find\nrace:uf_unite\nrace:atomicMin\n")
     env = dict(os.environ, LD_PRELOAD=tsan, TSAN_OPTIONS=f"report_signal_unsafe=0 history_size=4 exitcode=0 suppressions={supp}")
-    for extra in ([], ["crowded"], ["phased", "crowded"]):
+    for extra in ([], ["crowded"]):
         r = subprocess.run([shutil.which("python") or "python", os.path.join(HC, "tsan_fused_run.py"), ROOT, lib, "pipe_c4_m4"] + extra,
                            capture_output=True, text=True, env=env, timeout=280)
         out = r.stdout + r.stderr
@@ -464,30 +464,11 @@ def test_matcher_device_code_fuzz_vs_oracle(match_emu):
                 assert np.allclose(d["err"][b, :len(e)], e, rtol=1e-6, atol=1e-9)
 
 
-# ------------------------------------------------- the phase-synchronous variant (MOCAP_PIPELINE=phased, opt-in)
-@pytest.mark.parametrize("name", PIPE_CASES)
-def test_phased_kernel_on_host_vs_reference_golden(fused_emu, name):
-    """k_pipeline_phased (csrc/fused_phased.cuh): images and frame-sets are queued per CTA and the CTA changes
-    phase as a whole.  Same golden results as the single-pass kernel, every counter re-armed after a run."""
-    B = 12 if name != "pipe_c8_m16" else 6
-    z = load_golden(name, n=B)
-    d = fused_emu(z["frames"][:B], z["K"], z["R"], z["t"], runs=2, phased=1)
-    assert d["deferred_images"] == [] and d["deferred_sets"] == [] and d["dirty_scratch"] == 0
-    assert np.array_equal(d["blob_n"], z["blob_n"][:B])
-    assert np.array_equal(d["n"], z["nroot"][:B]) and not d["flags"].any()
-    for b in range(B):
-        for c in range(d["blob_n"].shape[1]):
-            k = d["blob_n"][b, c]
-            assert np.array_equal(d["blob_xy"][b, c, :k], z["blob_xy"][b, c, :k])
-        k = d["n"][b]
-        if k:
-            assert np.abs(d["obj"][b, :k] - z["obj"][b, :k]).max() <= X_TOL
-            assert np.allclose(d["err"][b, :k], z["err"][b, :k], rtol=ERR_RTOL, atol=1e-12)
-
-
-def test_phased_kernel_on_host_equals_single_pass_kernel(fused_emu):
-    """Bit-identical outputs of the two kernels on ragged geometry, many small frame-sets (the queues wrap several
-    times) and a crowded image (deferral to the worklists)."""
+def test_single_pass_kernel_on_host_defers_exactly_the_holed_images(fused_emu, blob_emu, match_emu):
+    """Many small frame-sets on ragged geometry: the kernel defers exactly the images that hold a blob with a hole
+    (RETR_TREE work, blob_holes.cuh) and their frame-sets, leaves no scratch word set, and finishes every other image
+    and frame-set as the separately driven blob and matcher device code do; a crowded image is deferred with 4 warps too."""
+    import cv2
     rng = np.random.default_rng(5)
     W, H, C, B = 48, 32, 3, 40
     frames = rng.integers(0, 40, size=(B, C, H, W), dtype=np.uint8)
@@ -499,27 +480,32 @@ def test_phased_kernel_on_host_equals_single_pass_kernel(fused_emu):
                 frames[b, c] = np.maximum(frames[b, c], (255 * np.exp(-((yy - cy) ** 2 + (xx - cx) ** 2) / (2 * sg * sg))).astype(np.uint8))
     K = np.array([[W * 1.0, 0, W / 2.0], [0, W * 1.0, H / 2.0], [0, 0, 1]])
     R = np.stack([np.eye(3)] * C); t = np.array([[-0.3 * c, 0.0, 0.0] for c in range(C)])
-    a = fused_emu(frames, K, R, t, max_roots=32, runs=2, phased=0)
-    b = fused_emu(frames, K, R, t, max_roots=32, runs=2, phased=1)
-    # the only images that may leave the fast path are the ones holding a blob with a hole (RETR_TREE work, blob_holes.cuh)
-    import cv2
+    d = fused_emu(frames, K, R, t, max_roots=32, runs=2)
     holed = []
     for i, img in enumerate(frames.reshape(B * C, H, W)):
         _, hier = cv2.findContours(cv2.threshold(img, 255 * 0.2, 255, cv2.THRESH_BINARY)[1], cv2.RETR_TREE, cv2.CHAIN_APPROX_SIMPLE)
         if hier is not None and (hier[0, :, 3] >= 0).any():
             holed.append(i)
-    assert b["dirty_scratch"] == 0 and b["deferred_images"] == holed and b["deferred_sets"] == sorted({i // C for i in holed})
-    assert np.array_equal(a["blob_n"], b["blob_n"]) and np.array_equal(a["blob_xy"], b["blob_xy"])
-    assert np.array_equal(a["n"], b["n"]) and np.array_equal(a["flags"], b["flags"])
-    for s in range(B):
-        k = a["n"][s]
-        assert np.array_equal(a["obj"][s, :k], b["obj"][s, :k]) and np.array_equal(a["err"][s, :k], b["err"][s, :k])
+    deferred_sets = sorted({i // C for i in holed})
+    assert d["dirty_scratch"] == 0 and d["deferred_images"] == holed and d["deferred_sets"] == deferred_sets
+    xy = np.zeros((B, C, 64, 2), np.int32); n = np.zeros((B, C), np.int32)
+    for b in range(B):
+        for c in range(C):
+            if b * C + c not in holed:
+                s1 = blob_emu(frames[b, c], seed=b)
+                n[b, c] = s1["n"]; xy[b, c, :s1["n"]] = s1["xy"]
+                assert d["blob_n"][b, c] == n[b, c] and np.array_equal(d["blob_xy"][b, c], xy[b, c]), (b, c)
+    m = match_emu(K, R, t, xy, n, max_roots=32)
+    for s in set(range(B)) - set(deferred_sets):
+        k = m["n"][s]
+        assert d["n"][s] == k and d["flags"][s] == m["flags"][s], s
+        assert np.array_equal(d["obj"][s, :k], m["obj"][s, :k]) and np.array_equal(d["err"][s, :k], m["err"][s, :k]), s
     z = load_golden("pipe_c4_m4", n=6)
     crowded = z["frames"][:6].copy()
     for k in range(70):
         y, x = 10 + 6 * (k // 35), 20 + 16 * (k % 35)
         crowded[2, 1, y:y + 3, x:x + 3] = 255
-    d = fused_emu(crowded, z["K"], z["R"], z["t"], runs=1, phased=1)
+    d = fused_emu(crowded, z["K"], z["R"], z["t"], n_warps=4, runs=1)
     assert d["deferred_images"] == [2 * 4 + 1] and d["deferred_sets"] == [2] and d["dirty_scratch"] == 0
     for s in (0, 1, 3, 4, 5):
         k = d["n"][s]

@@ -322,10 +322,10 @@ def _same_bits(a, b):
 @pytest.mark.parametrize("C,B", [(2, 18), (4, 12), (8, 9)])
 def test_holed_frame_sets_through_every_pipeline(torch, C, B):
     """Frame-sets whose images hold ring markers (an outer and a hole contour, often with the same centre: the matcher's
-    epipolar distances tie exactly), solid frame-sets and one flagged frame-set, through the single-pass kernel, the
-    three-kernel pipeline and the phase-synchronous variant (MOCAP_PIPELINE = fused | split | phased), with the winners'
-    pixels, and through the host entry point: counts, points, errors, flags and winners' pixels equal the oracle's
-    find_dot + match_and_triangulate per frame-set; the pipelines agree bit for bit, and so does a second call."""
+    epipolar distances tie exactly), solid frame-sets and one flagged frame-set, through the single-pass kernel and the
+    three-kernel pipeline (MOCAP_PIPELINE = fused | split), with the winners' pixels, and through the host entry point:
+    counts, points, errors, flags and winners' pixels equal the oracle's find_dot + match_and_triangulate per frame-set;
+    the pipelines agree bit for bit, and so does a second call."""
     from oracle.ref_port import RefPort
     rng = np.random.default_rng(40 + C)
     poses, K = synth.make_rig(C)
@@ -334,7 +334,7 @@ def test_holed_frame_sets_through_every_pipeline(torch, C, B):
     assert sum(len(r[0]) for r in ref) >= B and ref[B // 2][3] == F_HOLES
     batch = torch.from_numpy(frames).cuda()
     results = {}
-    for mode in ("fused", "split", "phased"):
+    for mode in ("fused", "split"):
         os.environ["MOCAP_PIPELINE"] = mode
         try:
             ctx = pkg.MocapContext(C, 640, 480, max_blobs=64, max_roots=128, max_cands=16, max_groups=1 << 16, max_segments=4096)
@@ -351,7 +351,7 @@ def test_holed_frame_sets_through_every_pipeline(torch, C, B):
         host = ctx.pipeline_host(frames)
         assert _same_bits({k: v.numpy() for k, v in host.items()}, runs[0]), mode
         results[mode] = runs[0]
-    assert _same_bits(results["fused"], results["split"]) and _same_bits(results["fused"], results["phased"])
+    assert _same_bits(results["fused"], results["split"])
 
 
 # ---------------------------------------------------------------------------------------- raw frames

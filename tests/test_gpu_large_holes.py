@@ -137,8 +137,8 @@ def _large_ring_sets(rng, C, B, poses, K):
 
 @pytest.mark.parametrize("C,B", [(2, 16), (4, 10), (8, 8)])
 def test_large_rings_through_every_pipeline(torch, C, B):
-    """Frame-sets with rings of 70-240 px beside ring markers, with the window on, through the single-pass kernel, the
-    three-kernel pipeline and the phase-synchronous variant, with the winners' pixels, and through the host entry point:
+    """Frame-sets with rings of 70-240 px beside ring markers, with the window on, through the single-pass kernel and the
+    three-kernel pipeline, with the winners' pixels, and through the host entry point:
     equal to the oracle's find_dot + match_and_triangulate per frame-set (cv2's lists), bit-equal across pipelines."""
     from oracle.ref_port import RefPort
     rng = np.random.default_rng(140 + C)
@@ -157,7 +157,7 @@ def test_large_rings_through_every_pipeline(torch, C, B):
     assert large >= B // 3
     batch = torch.from_numpy(frames).cuda()
     results = {}
-    for mode in ("fused", "split", "phased"):
+    for mode in ("fused", "split"):
         os.environ["MOCAP_PIPELINE"] = mode
         try:
             ctx = pkg.MocapContext(C, 640, 480, max_blobs=64, max_roots=128, max_cands=16, max_groups=1 << 16, max_segments=4096)
@@ -172,7 +172,7 @@ def test_large_rings_through_every_pipeline(torch, C, B):
         host = ctx.pipeline_host(frames)
         assert _same_bits({k: v.numpy() for k, v in host.items()}, run), mode
         results[mode] = run
-    assert _same_bits(results["fused"], results["split"]) and _same_bits(results["fused"], results["phased"])
+    assert _same_bits(results["fused"], results["split"])
 
 
 def test_raw_frames_with_large_ring_markers_vs_oracle_chain(torch):

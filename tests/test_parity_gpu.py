@@ -935,50 +935,6 @@ def test_matcher_heavy_fuzz_8_cameras(torch):
         assert np.allclose(err[b, :cnt[b]], e, rtol=1e-6, atol=1e-9)
 
 
-@pytest.mark.skipif(__import__("os").environ.get("MOCAP_TEST_TMA") != "1",
-                    reason="experimental bulk-copy variant (not the default pipeline): run with MOCAP_TEST_TMA=1")
-def test_tma_pipeline_agrees_with_fused(torch, monkeypatch):
-    """MOCAP_PIPELINE=tma (bulk-copy ring kernel) against the default fused kernel: identical bits, including
-    deferred images / frame-sets and a second pass on the same context; also on a ragged image size."""
-    z = load_golden("pipe_c4_m4")
-    C = 4
-    frames = z["frames"][:12].copy()
-    frames[1, 2, 100:160, 40:600] = 255
-    frames[5, 0, 300:304, 100:400] = 255
-    res = {}
-    for mode in ("fused", "tma"):
-        monkeypatch.setenv("MOCAP_PIPELINE", mode)
-        ctx = _ctx(C, max_blobs=64, max_roots=64, max_segments=4096)
-        ctx.set_cameras([z["K"]] * C, poses_from(z))
-        big = torch.from_numpy(np.concatenate([frames] * 40)).cuda()        # 480 frame-sets: every CTA gets work
-        out = ctx.pipeline(big)
-        torch.cuda.synchronize()
-        res[mode] = {k: v.cpu().numpy().copy() for k, v in out.items()}
-        out2 = ctx.pipeline(big)
-        torch.cuda.synchronize()
-        assert np.array_equal(out2["n"].cpu().numpy(), res[mode]["n"])
-    a, b = res["fused"], res["tma"]
-    assert np.array_equal(a["n"], b["n"]) and np.array_equal(a["flags"], b["flags"])
-    mask = np.arange(a["obj"].shape[1])[None, :] < a["n"][:, None]
-    assert np.array_equal(a["obj"][mask], b["obj"][mask]) and np.array_equal(a["err"][mask], b["err"][mask])
-    # ragged chunks: 320x320 -> 6400 segments = 50 chunks of 128
-    rng = np.random.default_rng(5)
-    small = rng.integers(0, 40, size=(30, 2, 320, 320), dtype=np.uint8)
-    small[:, :, 100:104, 50:58] = 255
-    small[:, 1, 200:204, 150:158] = 255
-    K = np.array([[300.0, 0, 160], [0, 300, 160], [0, 0, 1]])
-    poses = [{"R": np.eye(3), "t": np.zeros(3)}, {"R": np.eye(3), "t": np.array([-0.3, 0, 0])}]
-    r2 = {}
-    for mode in ("fused", "tma"):
-        monkeypatch.setenv("MOCAP_PIPELINE", mode)
-        ctx = pkg.MocapContext(2, 320, 320, max_roots=16)
-        ctx.set_cameras([K, K], poses)
-        out = ctx.pipeline(torch.from_numpy(small).cuda())
-        torch.cuda.synchronize()
-        r2[mode] = {k: v.cpu().numpy().copy() for k, v in out.items()}
-    assert np.array_equal(r2["fused"]["n"], r2["tma"]["n"]) and (r2["tma"]["n"] > 0).all()
-
-
 def test_install_into_patches_a_helpers_like_module(torch):
     """install_into() on a stand-in for the reference's helpers module (same attribute surface: the Cameras
     singleton with camera_params, and the module-level hot-path functions): afterwards the module's own names
@@ -1070,29 +1026,6 @@ def test_heavy_batches_take_the_three_kernel_pipeline(torch, monkeypatch):
             for b in range(len(n)):
                 assert np.array_equal(o["obj"][b, :n[b]], outs[0]["obj"][b, :n[b]])
                 assert np.array_equal(o["err"][b, :n[b]], outs[0]["err"][b, :n[b]])
-
-
-@pytest.mark.skipif(__import__("os").environ.get("MOCAP_TEST_PHASED") != "1",
-                    reason="phase-synchronous variant of the single-pass kernel: opt-in until it has been measured (MOCAP_TEST_PHASED=1)")
-@pytest.mark.parametrize("name", PIPE_CASES)
-def test_phased_pipeline_agrees_with_fused(torch, monkeypatch, name):
-    """MOCAP_PIPELINE=phased against the default single-pass kernel: identical bits, twice on the same context."""
-    z = load_golden(name)
-    C = int(z["C"])
-    results = {}
-    for mode in ("fused", "phased"):
-        monkeypatch.setenv("MOCAP_PIPELINE", mode)
-        ctx = _ctx(C, max_blobs=64, max_roots=128)
-        ctx.set_cameras([z["K"]] * C, poses_from(z))
-        for _ in range(2):
-            out = ctx.pipeline(torch.from_numpy(z["frames"]).cuda())
-            torch.cuda.synchronize()
-        results[mode] = {k: v.cpu().numpy().copy() for k, v in out.items()}
-    n = results["fused"]["n"]
-    assert np.array_equal(results["phased"]["n"], n) and np.array_equal(n, z["nroot"])
-    for b in range(len(n)):
-        assert np.array_equal(results["phased"]["obj"][b, :n[b]], results["fused"]["obj"][b, :n[b]])
-        assert np.array_equal(results["phased"]["err"][b, :n[b]], results["fused"]["err"][b, :n[b]])
 
 
 # ---------------------------------------------------------------------------------------------------------------
