@@ -250,7 +250,8 @@ MOCAP_API int  mocap_track_objects_gated_dev(mocap_tracker* tr, const double* ob
  *   this context, and timestamps).  Any other combination returns MOCAP_EINVAL before any launch.
  *   raw uint8 [n_reads][n_cam][in_h][in_w][3]; timestamps double [n_reads] (the clock reading of each read, locate
  *   mode only, may be NULL otherwise); frames uint8 [n_reads][n_cam][S][S][3] or NULL: the processed frames, with a
- *   1-px (100, 255, 100) dot at every blob centre when CAPTURE is set (what the drop-in _find_dot draws).
+ *   1-px (100, 255, 100) dot at every blob centre when CAPTURE is set (what the drop-in _find_dot draws), or the whole
+ *   detection overlay when the context draws it (mocap_set_overlay).
  *   result: ONE device buffer of mocap_live_layout(ctx, n_reads, tr ? num_objects : 0).total bytes, struct of arrays
  *   over the reads, each slice written by the stage that computes it (byte offsets in mocap_live_layout):
  *     flags      int32  [R]          OR of the read's images' MOCAP_F_* bits and its frame-set flags
@@ -287,6 +288,35 @@ MOCAP_API int  mocap_live_dev(mocap_ctx* ctx, mocap_tracker* tr, const uint8_t* 
  * (if asked for), one synchronisation. */
 MOCAP_API int  mocap_live_host(mocap_ctx* ctx, mocap_tracker* tr, const uint8_t* raw, int n_reads, int mode,
                                const double* timestamps, uint8_t* frames, void* result);
+
+/* The detection overlay the reference draws into the frames it returns, byte for byte as cv2 draws it.
+ * _find_dot (helpers.py:148,156-157), in every mode with CAPTURE: the contour of every blob and hole of the thresholded
+ * grey in (0, 255, 0) -- the foreground pixels (grey > 51 of the undrawn frame) with a background or outside
+ * 4-neighbour, which is what cv.drawContours(findContours(RETR_TREE, CHAIN_APPROX_SIMPLE)) paints -- then per blob
+ * centre (x, y) the label cv.putText('(x, y)', (x, y - 15), FONT_HERSHEY_SIMPLEX, 0.3, (100, 255, 100), 1) and
+ * cv.circle((x, y), 1, (100, 255, 100), -1), a 5-pixel plus.
+ * find_point_correspondance_and_object_points (helpers.py:359-365, drawlines :497-504), with TRIANGULATE as well: into
+ * camera i >= 1, the epipolar line of every root that exists before camera i, camera by camera and roots in creation
+ * order, from (0, int(-c/b)) to (width, int(-(c + a*width)/b)) in float32 arithmetic, cv.line thickness 1, LINE_8.
+ * The reference colours each line with np.random.randint(0, 255, 3); here line n since mocap_set_overlay gets entry
+ * n % palette_len of np.random.RandomState(seed).randint(0, 255, (palette_len, 3)), which for the first palette_len
+ * lines is the reference's colour after np.random.seed(seed).  A line where the reference raises -- b == 0, a
+ * non-finite end point, or one outside 32 bits -- is skipped (it still takes its colour).
+ * mocap_set_overlay: on != 0 makes mocap_live_dev, mocap_live_host and mocap_live_jpeg_host draw the overlay into the
+ *   frames they return or encode; on == 0 (the default) returns them to the 1-px dots.  Their other outputs do not
+ *   change.  Builds the palette (palette_len 1..MOCAP_OVERLAY_MAX_PALETTE, else MOCAP_EINVAL) and resets the line
+ *   counter to 0.  Synchronises the context's stream.
+ * mocap_overlay_dev: the overlay of frames that did not come through the live loop, in place: frames uint8
+ *   [n_sets][n_cam][height][width][3] of the context's size, undrawn; blob_xy int32 [n_sets][n_cam][max_blobs][2] and
+ *   blob_n int32 [n_sets][n_cam] as mocap_detect_dev leaves them (the first min(blob_n, max_blobs) centres are used).
+ *   mode: MOCAP_LIVE_CAPTURE draws _find_dot's layers, MOCAP_LIVE_TRIANGULATE the epipolar lines (needs
+ *   mocap_set_cameras and mocap_set_overlay; moves the line counter on), both for both.  Draws whether or not the
+ *   context's overlay is on.  DEVICE pointers, the context's stream, never synchronises; CAPTURE uses 1 byte of the
+ *   context's scratch per pixel of a group of up to 64 MiB of grey plane (192 MiB of frames). */
+#define MOCAP_OVERLAY_MAX_PALETTE 65536
+MOCAP_API int  mocap_set_overlay(mocap_ctx* ctx, int on, uint32_t seed, int palette_len);
+MOCAP_API int  mocap_overlay_dev(mocap_ctx* ctx, uint8_t* frames, int n_sets, const int32_t* blob_xy, const int32_t* blob_n,
+                                 int mode);
 
 /* Baseline JPEG encoding -- the camera stream's cv.imencode('.jpg', frames) (index.py:55-56), byte for byte what
  * cv2.imencode('.jpg', img, [cv2.IMWRITE_JPEG_QUALITY, quality]) returns with libjpeg-turbo: 3-channel BGR input,

@@ -114,6 +114,8 @@ SYMBOLS = {
     "mocap_live_layout": (C.c_int, [_P, C.c_int, C.c_int, C.POINTER(LiveLayout)]),
     "mocap_live_dev": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P, _P, _P]),
     "mocap_live_host": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P, _P, _P]),
+    "mocap_set_overlay": (C.c_int, [_P, C.c_int, C.c_uint32, C.c_int]),
+    "mocap_overlay_dev": (C.c_int, [_P, _P, C.c_int, _P, _P, C.c_int]),
     "mocap_jpeg_bound": (C.c_uint64, [C.c_int, C.c_int]),
     "mocap_encode_jpeg_dev": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, C.c_uint64, _P]),
     "mocap_live_jpeg_host": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P, _P, _P, C.c_int, _P, C.c_uint64, _P]),

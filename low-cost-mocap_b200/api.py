@@ -95,6 +95,7 @@ class MocapContext:
         self._tdev = None
         self._pp_in = None
         self.large_holes = False
+        self.overlay_on = False
 
     # -- lifetime -------------------------------------------------------------------------
     def close(self):
@@ -130,6 +131,38 @@ class MocapContext:
         (mocap_set_large_holes, include/mocap_b200.h)."""
         self._check(self.lib.mocap_set_large_holes(self.h, 1 if on else 0))
         self.large_holes = bool(on)
+
+    def set_overlay(self, on=True, seed=0, palette_len=65536):
+        """Draw the detection overlay into the frames ``live`` and ``live_host`` return or encode, byte for byte as cv2
+        draws it (mocap_set_overlay, include/mocap_b200.h).  In every mode with LIVE_CAPTURE, _find_dot's drawing
+        (helpers.py:148,156-157): the contours of the thresholded grey in (0, 255, 0), then a '(x, y)' label and a
+        5-pixel plus in (100, 255, 100) at every blob centre.  With LIVE_TRIANGULATE too, the matcher's epipolar lines
+        (helpers.py:365): line n since this call in colour n % palette_len of
+        np.random.RandomState(seed).randint(0, 255, (palette_len, 3)), the reference's colours after np.random.seed(seed)
+        for the first palette_len lines; a line the reference would crash on is skipped.  Off (the default) the frames
+        carry 1-px centre dots; nothing else they return changes.  Resets the line counter."""
+        self._check(self.lib.mocap_set_overlay(self.h, 1 if on else 0, int(seed) & 0xffffffff, int(palette_len)))
+        self.overlay_on = bool(on)
+
+    def overlay(self, frames, xy, n, mode=LIVE_CAPTURE):
+        """Draw the overlay into undrawn frames in place (mocap_overlay_dev): frames a contiguous uint8 cuda tensor of
+        frame-sets [..., n_cam, H, W, 3] of this context's size, xy int32 [n_sets * n_cam, max_blobs, 2] / n int32
+        [n_sets * n_cam] their blob lists (``detect``'s).  mode: LIVE_CAPTURE for _find_dot's layers, LIVE_TRIANGULATE for
+        the epipolar lines (needs ``set_cameras`` and ``set_overlay``), or both.  Draws whether or not ``set_overlay`` is
+        on.  No synchronisation."""
+        torch = _torch()
+        per = self.n_cam * self.height * self.width * 3
+        if frames.dtype != torch.uint8 or not frames.is_cuda or not frames.is_contiguous() or frames.dim() < 3 \
+                or tuple(frames.shape[-3:]) != (self.height, self.width, 3) or frames.numel() % per:
+            raise ValueError(f"overlay: frames must be a contiguous uint8 cuda tensor of frame-sets [..., {self.n_cam}, {self.height}, "
+                             f"{self.width}, 3]")
+        k = frames.numel() // per
+        if xy.numel() != k * self.n_cam * self.cfg.max_blobs * 2 or n.numel() != k * self.n_cam or xy.dtype != torch.int32 \
+                or n.dtype != torch.int32:
+            raise ValueError(f"overlay: xy must be int32 [{k * self.n_cam}, {self.cfg.max_blobs}, 2] and n int32 [{k * self.n_cam}] (detect's)")
+        self.use_current_stream()
+        self._check(self.lib.mocap_overlay_dev(self.h, _ptr(frames), k, _ptr(xy.contiguous()), _ptr(n.contiguous()), int(mode)))
+        return frames
 
     def set_cameras(self, intrinsics, poses):
         """intrinsics: C 3x3 matrices; poses: list of {"R": 3x3, "t": 3} as the reference passes them."""
@@ -780,12 +813,17 @@ class MocapSession:
 
     _default = None
 
-    def __init__(self, intrinsics, width=640, height=480, device=0, large_holes=False):
+    def __init__(self, intrinsics, width=640, height=480, device=0, large_holes=False, overlay=False, overlay_seed=0):
         """``large_holes``: the contexts the session creates reproduce holed blobs wider or taller than 62 pixels as
-        cv2 does (MocapContext.set_large_holes); off, find_dot raises on a frame with one."""
+        cv2 does (MocapContext.set_large_holes); off, find_dot raises on a frame with one.  ``overlay``: find_dot and
+        camera_read draw the detection overlay _find_dot draws instead of 1-px centre dots, and
+        find_point_correspondance_and_object_points and camera_read the epipolar lines, in the colours of
+        np.random.seed(overlay_seed) (MocapContext.set_overlay)."""
         self.intrinsics = [np.asarray(k, dtype=np.float64).reshape(3, 3) for k in intrinsics]
         self.width, self.height, self.device = width, height, device
         self.large_holes = bool(large_holes)
+        self.overlay = bool(overlay)
+        self.overlay_seed = int(overlay_seed)
         self._ctxs = {}
         self._live = {}
         self._lock = threading.RLock()
@@ -823,12 +861,15 @@ class MocapSession:
 def find_dot(img, session=None):
     """Mirror of ``Cameras._find_dot(self, img)`` (helpers.py:143-163): returns
     ``(img, image_points)`` with image_points a list of ``[x, y]`` or ``[[None, None]]``.
-    The contour / text overlay the reference draws into ``img`` (helpers.py:148,156-157) is
-    cosmetic and is not reproduced; a 1-px centre dot is drawn instead."""
+    With the session's ``overlay`` the contours, labels and plus marks the reference draws into
+    ``img`` (helpers.py:148,156-157) are drawn as cv2 draws them (``img`` must then be H x W x 3, as
+    the reference's cvtColor needs); without it a 1-px centre dot is drawn instead."""
     torch = _torch()
     s = session or MocapSession.default()
     img = np.ascontiguousarray(img, dtype=np.uint8)
     h, w = img.shape[:2]
+    if s.overlay and (img.ndim != 3 or img.shape[2] != 3):
+        raise ValueError(f"find_dot: the overlay needs an H x W x 3 frame (got {img.shape})")
     with s._lock:
         ctx = s._ctxs.get(("detect", w, h))
         if ctx is None:
@@ -837,10 +878,15 @@ def find_dot(img, session=None):
             if s.large_holes:
                 ctx.set_large_holes(True)
             s._ctxs[("detect", w, h)] = ctx
-        d = ctx.detect(torch.from_numpy(img).to(ctx.torch_device))
+        frame = torch.from_numpy(img).to(ctx.torch_device)
+        d = ctx.detect(frame)
         raise_on_overflow(d["flags"][0].item(), "find_dot")
         n = int(d["n"][0].item())
         pts = d["xy"][0, :n].cpu().numpy().tolist()
+        if s.overlay:
+            img[...] = ctx.overlay(frame, d["xy"], d["n"], LIVE_CAPTURE).cpu().numpy()
+    if s.overlay:
+        return img, (pts if pts else [[None, None]])
     for x, y in pts:
         if 0 <= y < h and 0 <= x < w:
             img[y, x] = (100, 255, 100) if img.ndim == 3 else 255
@@ -891,8 +937,9 @@ def calculate_reprojection_error(image_points, object_point, camera_poses, sessi
 def find_point_correspondance_and_object_points(image_points, camera_poses, frames, session=None):
     """Mirror of helpers.py:339-421: returns ``(errors (K,), object_points (K,3), frames)``.
     Like the reference it removes the ``[None, None]`` sentinels from ``image_points`` in
-    place (helpers.py:342-346); the epipolar lines the reference draws into ``frames``
-    (helpers.py:365) are cosmetic and are not drawn."""
+    place (helpers.py:342-346).  With the session's ``overlay`` the epipolar lines the reference draws
+    into ``frames`` (helpers.py:365) are drawn in place, as cv2 draws them, in the colours of
+    ``MocapContext.set_overlay`` (the session's lines counted from its first call); without it they are not."""
     torch = _torch()
     s = session or MocapSession.default()
     for pts in image_points:
@@ -918,7 +965,32 @@ def find_point_correspondance_and_object_points(image_points, camera_poses, fram
         k = int(d["n"][0].item())
         errors = d["err"][0, :k].cpu().numpy()
         object_points = d["obj"][0, :k].cpu().numpy()
+        if s.overlay:
+            _draw_epilines(s, camera_poses, frames, xy, n)
     return errors, object_points, frames
+
+
+def _draw_epilines(s, camera_poses, frames, xy, n):
+    """The epipolar lines of find_point_correspondance_and_object_points into ``frames`` (C arrays H x W x 3), in place,
+    on a context of the frames' size that keeps the session's line counter."""
+    torch = _torch()
+    n_cam = len(camera_poses)
+    shape = tuple(np.shape(frames[0]))
+    if len(frames) != n_cam or any(tuple(np.shape(f)) != shape for f in frames) or len(shape) != 3 or shape[2] != 3:
+        raise ValueError(f"find_point_correspondance_and_object_points: the overlay needs {n_cam} frames of one H x W x 3 size")
+    key = ("epilines", n_cam, shape[1], shape[0])
+    ctx = s._ctxs.get(key)
+    if ctx is None:
+        ctx = MocapContext(n_cam, shape[1], shape[0], s.device, **MIRROR_LIMITS)
+        ctx.set_overlay(False, s.overlay_seed)
+        s._ctxs[key] = ctx
+    ctx.set_cameras(s.intrinsics[:n_cam], camera_poses)
+    dev = ctx.torch_device
+    t = torch.from_numpy(np.ascontiguousarray(np.stack([np.asarray(f, dtype=np.uint8) for f in frames]))).to(dev)
+    ctx.overlay(t, torch.from_numpy(xy).to(dev), torch.from_numpy(n).to(dev), LIVE_TRIANGULATE)
+    out = t.cpu().numpy()
+    for i in range(1, n_cam):
+        frames[i][...] = out[i]
 
 
 def locate_objects(object_points, errors, session=None):
@@ -1106,6 +1178,8 @@ def _live_cameras(cams, s, frames):
     ctx = MocapContext(C_, S, S, s.device, **MIRROR_LIMITS)
     if s.large_holes:
         ctx.set_large_holes(True)
+    if s.overlay:
+        ctx.set_overlay(True, s.overlay_seed)
     ctx.set_preprocess(in_w, in_h, rot, [np.asarray(p["intrinsic_matrix"], dtype=np.float64) for p in params],
                        [np.asarray(p["distortion_coef"], dtype=np.float64).reshape(-1)[:5] for p in params])
     if st is not None:
@@ -1119,7 +1193,7 @@ def camera_read(cams, session=None, clock=time.time, jpeg=None):
     one ``live_host`` call whose mode follows ``is_capturing_points`` / ``is_triangulating_points`` /
     ``is_locating_objects`` as the reference nests them, then the reference's emits and serial writes
     (:func:`live_read_events`).  Returns the processed frames -- with the centre dots while capturing -- in the container
-    type the driver gave.  The context is built from ``camera_params`` and the first read's size; poses and the world
+    type the driver gave (with the session's ``overlay``, the detection overlay instead of the dots).  The context is built from ``camera_params`` and the first read's size; poses and the world
     matrix are re-sent only when their values change; a new ``kalman_filter`` object (start_trangulating_points) starts
     a fresh device tracker, which reads ``clock`` once per read.  The filter object itself is never called.
     ``jpeg`` (a quality, 1..100): the same call also encodes the frames side by side on the device as
@@ -1223,7 +1297,8 @@ PATCHED_NAMES = ("triangulate_point", "triangulate_points", "calculate_reproject
                  "bundle_adjustment", "locate_objects")
 
 
-def install_into(helpers_module, *also, session=None, tracker=False, large_holes=False, live=False, stream=False):
+def install_into(helpers_module, *also, session=None, tracker=False, large_holes=False, live=False, stream=False, overlay=False,
+                 overlay_seed=0):
     """Point a loaded reference ``helpers`` module at the CUDA path (INTEGRATION.md).
 
     ``also``: modules that imported the hot-path names BY VALUE -- the reference's ``index.py`` does
@@ -1249,12 +1324,20 @@ def install_into(helpers_module, *also, session=None, tracker=False, large_holes
     ``get_frames`` returns np.hstack of the read's frames as a :class:`StreamFrames` carrying the JPEG the device made of
     them at cv2's default quality, and ``cv`` in every module of ``also`` that holds it is re-bound to a
     :class:`StreamCv` proxy, whose ``imencode('.jpg', frames)`` returns those bytes -- cv2's, byte for byte -- and hands
-    every other call to cv2."""
+    every other call to cv2.
+
+    ``overlay=True``: the session made here draws what the reference draws into its frames, as cv2 draws it, where the
+    drop-in draws 1-px centre dots by default: ``_find_dot``'s contours, '(x, y)' labels and plus marks, and the
+    epipolar lines of ``find_point_correspondance_and_object_points`` in the colours of np.random.seed(overlay_seed)
+    (MocapContext.set_overlay); with ``live=True`` into the frames ``_camera_read`` returns and the stream's JPEG.  A
+    ``session`` passed in keeps its own settings; asking for an overlay it does not draw raises ValueError."""
+    if session is not None and overlay and not session.overlay:
+        raise ValueError("install_into: overlay=True with a session made without overlay (MocapSession(..., overlay=True))")
     if stream and not live:
         raise ValueError("install_into: stream=True needs live=True (the JPEG is made in the live read's device call)")
     cams = helpers_module.Cameras.instance()
     s = session or MocapSession.install([np.asarray(p["intrinsic_matrix"], dtype=np.float64) for p in cams.camera_params],
-                                        large_holes=large_holes)
+                                        large_holes=large_holes, overlay=overlay, overlay_seed=overlay_seed)
     # helpers.Cameras is a Singleton WRAPPER object (Singleton.py:17-37); _camera_read looks _find_dot up on the
     # decorated class of the instance, so that is where the replacement goes
     type(cams)._find_dot = lambda self, img: find_dot(img, s)

@@ -7,7 +7,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libmocap_b200.so")
-SOURCES = ["api.cu", "blob_kernels.cu", "match_kernels.cu", "fused_kernel.cu", "locate_kernels.cu", "preproc.cu", "calib_init.cu", "calib_ransac.cu", "calib_graph.cu", "ba.cu", "ba_dev.cu", "screen.cu", "track.cu", "live.cu", "jpeg.cu"]
+SOURCES = ["api.cu", "blob_kernels.cu", "match_kernels.cu", "fused_kernel.cu", "locate_kernels.cu", "preproc.cu", "calib_init.cu", "calib_ransac.cu", "calib_graph.cu", "ba.cu", "ba_dev.cu", "screen.cu", "track.cu", "live.cu", "jpeg.cu", "overlay.cu"]
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = GENCODE + ["-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--use_fast_math=false"]

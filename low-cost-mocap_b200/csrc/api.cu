@@ -187,6 +187,7 @@ void mocap_destroy(mocap_ctx* ctx) {
     cudaFree(ctx->d_match_items); cudaFree(ctx->d_match_partial); cudaFree(ctx->d_match_range); cudaFree(ctx->d_match_arrive);
     cudaFree(ctx->d_pp_m1); cudaFree(ctx->d_pp_m2); cudaFree(ctx->d_pp_rot);
     cudaFree(ctx->d_live_in); cudaFree(ctx->d_live_out);
+    cudaFree(ctx->d_palette); cudaFree(ctx->d_line_counter); cudaFree(ctx->d_line_counts);
     if (ctx->h_live_in) cudaFreeHost(ctx->h_live_in);
     if (ctx->h_live_out) cudaFreeHost(ctx->h_live_out);
     jpeg_release(ctx);

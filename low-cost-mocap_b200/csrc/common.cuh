@@ -55,6 +55,10 @@ struct mocap_ctx {
     int32_t*  d_blob_xy;
     int32_t*  d_blob_n;
     int32_t*  d_img_flags;
+    int       overlay_on;       // mocap_set_overlay: the live entry points draw the detection overlay (overlay.cu)
+    uint8_t*  d_palette; int palette_len;          // the epipolar lines' colours [palette_len][3]
+    unsigned long long* d_line_counter;            // epipolar lines drawn since mocap_set_overlay
+    uint32_t* d_line_counts; int line_counts_cap;  // lines per frame-set of a launch group
     // host-path staging
     uint8_t*  d_stage[2];
     size_t    stage_bytes;
@@ -116,6 +120,10 @@ struct LiveOut {
     int mode;                   // MOCAP_LIVE_* bits
 };
 int launch_live_blobs(mocap_ctx* ctx, const LiveOut& live, int s0, int n_sets, int have_blobs, uint8_t* frames);
+// the detection overlay of n_images frames of the context's size from their grey planes and blob lists, and the
+// matcher's epipolar lines into n_sets frame-sets of them (overlay.cu)
+int launch_overlay(mocap_ctx* ctx, const uint8_t* gray, uint8_t* frames, int n_images, const int32_t* blob_xy, const int32_t* blob_n);
+int launch_epilines(mocap_ctx* ctx, uint8_t* frames, int n_sets, const int32_t* blob_xy, const int32_t* blob_n);
 // mocap_live_host in two halves (live.cu), so that mocap_live_jpeg_host runs the same chain: live_check; live_host_run
 // (staging in, the chain; the frames stay on the device when keep_frames); live_host_finish (result, frames and
 // extra_bytes of device data back, one synchronisation)

@@ -112,6 +112,19 @@ static __device__ __noinline__ void eval_group(const CameraTables* __restrict__ 
     err = mean_like_numpy(sq, 2 * nv, nv == C);
 }
 
+// cv.computeCorrespondEpilines of the float32 point (rx, ry) with F (helpers.py:362-364): double math, the float32 line
+// (a, b, c) returned as doubles.  The detection overlay draws the same lines (overlay.cu).
+__device__ __forceinline__ void epiline_f32(const double* F, double rx, double ry, double& a, double& b, double& c) {
+    a = DADD(DADD(DMUL(F[0], rx), DMUL(F[1], ry)), F[2]);
+    b = DADD(DADD(DMUL(F[3], rx), DMUL(F[4], ry)), F[5]);
+    c = DADD(DADD(DMUL(F[6], rx), DMUL(F[7], ry)), F[8]);
+    double nu = DADD(DMUL(a, a), DMUL(b, b));
+    nu = (nu != 0.0) ? 1.0 / sqrt(nu) : 1.0;
+    a = (double)(float)DMUL(a, nu);
+    b = (double)(float)DMUL(b, nu);
+    c = (double)(float)DMUL(c, nu);
+}
+
 // The matcher of one frame-set is three steps of one warp: prepare (roots, candidate lists, group counts), evaluate a
 // range of the frame-set's candidate groups (per-root best so far in shared memory), emit (winners in root order).
 // match_triangulate_warp runs them back to back; k_match_chunks (match_kernels.cu) gives the middle step of a frame-set
@@ -161,16 +174,8 @@ static __device__ __forceinline__ MatchPrep match_prepare_warp(
             const int rc = ws.rcam[j];
             const double rx = (double)xy[((size_t)rc * MB + ws.rpt[j]) * 2 + 0];
             const double ry = (double)xy[((size_t)rc * MB + ws.rpt[j]) * 2 + 1];
-            const double* F = tb->F[rc][i];
-            // cv.computeCorrespondEpilines on a float32 point: double math, float32 result (helpers.py:363-364)
-            double a = DADD(DADD(DMUL(F[0], rx), DMUL(F[1], ry)), F[2]);
-            double b = DADD(DADD(DMUL(F[3], rx), DMUL(F[4], ry)), F[5]);
-            double c = DADD(DADD(DMUL(F[6], rx), DMUL(F[7], ry)), F[8]);
-            double nu = DADD(DMUL(a, a), DMUL(b, b));
-            nu = (nu != 0.0) ? 1.0 / sqrt(nu) : 1.0;
-            a = (double)(float)DMUL(a, nu);
-            b = (double)(float)DMUL(b, nu);
-            c = (double)(float)DMUL(c, nu);
+            double a, b, c;
+            epiline_f32(tb->F[rc][i], rx, ry, a, b, c);
             const double den = sqrt(DADD(DMUL(a, a), DMUL(b, b)));      // helpers.py:373
             double dist[MOCAP_MAX_CANDS];
             uint8_t* cl = ws.cand + ((size_t)j * C + i) * KC;

@@ -126,7 +126,8 @@ static int launch_preprocess(mocap_ctx* ctx, const uint8_t* raw_frames, int n_im
 // on 1 byte per pixel through the single-pass pipeline kernel; the processed BGR frames are only written when the
 // caller asks for them.  stages: RAW_PREPROCESS, RAW_DETECT (+ S1, blob lists left in the context's d_blob_xy /
 // d_blob_n / d_img_flags) or RAW_MATCH (+ S2+S3 into obj / err / n_obj / set_flags, the blob lists left as well).
-// live != NULL: k_live_blobs after each group's S1 (live.cu).
+// live != NULL: k_live_blobs after each group's S1 (live.cu), and the detection overlay (overlay.cu) when the context
+// draws it.
 int run_raw_groups(mocap_ctx* ctx, const uint8_t* raw_frames, int n_frame_sets, int threshold, int stages, uint8_t* processed,
                    double* obj, double* err, int32_t* n_obj, int32_t* set_flags, const LiveOut* live) {
     const int C = ctx->cfg.n_cam, S = ctx->cfg.width;
@@ -149,6 +150,12 @@ int run_raw_groups(mocap_ctx* ctx, const uint8_t* raw_frames, int n_frame_sets, 
             st = launch_detect(ctx, gray, ns * C, 1, threshold, ctx->d_blob_xy, ctx->d_blob_n, nullptr, ctx->d_img_flags);
         if (st) return st;
         if (live && (st = launch_live_blobs(ctx, *live, s0, ns, stages != RAW_PREPROCESS, out)) != MOCAP_OK) return st;
+        // the overlay over k_live_blobs's dots, while this group's grey plane is still in the scratch
+        if (live && ctx->overlay_on && out && (live->mode & MOCAP_LIVE_CAPTURE)) {
+            if ((st = launch_overlay(ctx, gray, out, ns * C, ctx->d_blob_xy, ctx->d_blob_n)) != MOCAP_OK) return st;
+            if ((live->mode & MOCAP_LIVE_TRIANGULATE) && (st = launch_epilines(ctx, out, ns, ctx->d_blob_xy, ctx->d_blob_n)) != MOCAP_OK)
+                return st;
+        }
     }
     return MOCAP_OK;
 }
