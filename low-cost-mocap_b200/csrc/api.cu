@@ -22,56 +22,31 @@ int mocap_fail(mocap_ctx* ctx, int code, const char* fmt, ...) {
     return code;
 }
 
-int ensure_scratch(mocap_ctx* ctx, size_t bytes) {
-    if (bytes <= ctx->scratch_bytes) return MOCAP_OK;
-    CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-    cudaFree(ctx->d_scratch);
-    ctx->d_scratch = nullptr; ctx->scratch_bytes = 0;
-    CUDA_TRY(ctx, cudaMalloc(&ctx->d_scratch, bytes));
-    ctx->scratch_bytes = bytes;
-    return MOCAP_OK;
-}
-
-
 // ---- scratch management ------------------------------------------------------------------
 int ensure_images(mocap_ctx* ctx, int n_images) {
     if (n_images <= ctx->cap_images) return MOCAP_OK;
-    CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-    cudaFree(ctx->d_seg_count); cudaFree(ctx->d_seg_list); cudaFree(ctx->d_worklist); cudaFree(ctx->d_work_count); cudaFree(ctx->d_set_worklist); cudaFree(ctx->d_img_done); cudaFree(ctx->d_set_done); cudaFree(ctx->d_unit_counter); cudaFree(ctx->d_blob_xy); cudaFree(ctx->d_blob_n); cudaFree(ctx->d_img_flags);
-    ctx->d_seg_count = nullptr; ctx->d_seg_list = nullptr; ctx->d_worklist = nullptr; ctx->d_work_count = nullptr; ctx->d_set_worklist = nullptr; ctx->d_img_done = nullptr; ctx->d_set_done = nullptr; ctx->d_unit_counter = nullptr; ctx->d_blob_xy = nullptr; ctx->d_blob_n = nullptr; ctx->d_img_flags = nullptr;
-    ctx->cap_images = 0;
     const size_t n = (size_t)n_images;
-    CUDA_TRY(ctx, cudaMalloc(&ctx->d_seg_count, n * sizeof(uint32_t)));
-    CUDA_TRY(ctx, cudaMalloc(&ctx->d_seg_list, n * ctx->cfg.max_segments * sizeof(uint32_t)));
-    CUDA_TRY(ctx, cudaMalloc(&ctx->d_worklist, n * sizeof(uint32_t)));
-    CUDA_TRY(ctx, cudaMalloc(&ctx->d_work_count, 4 * sizeof(uint32_t)));
-    CUDA_TRY(ctx, cudaMemsetAsync(ctx->d_work_count, 0, 4 * sizeof(uint32_t), ctx->stream));
-    CUDA_TRY(ctx, cudaMalloc(&ctx->d_set_worklist, n * sizeof(uint32_t)));
-    CUDA_TRY(ctx, cudaMalloc(&ctx->d_img_done, n * sizeof(uint32_t)));
-    CUDA_TRY(ctx, cudaMalloc(&ctx->d_set_done, 2 * n * sizeof(uint32_t)));
-    CUDA_TRY(ctx, cudaMalloc(&ctx->d_unit_counter, sizeof(unsigned long long)));
-    CUDA_TRY(ctx, cudaMemsetAsync(ctx->d_img_done, 0, n * sizeof(uint32_t), ctx->stream));
-    CUDA_TRY(ctx, cudaMemsetAsync(ctx->d_set_done, 0, 2 * n * sizeof(uint32_t), ctx->stream));
-    CUDA_TRY(ctx, cudaMalloc(&ctx->d_blob_xy, n * ctx->cfg.max_blobs * 2 * sizeof(int32_t)));
-    CUDA_TRY(ctx, cudaMalloc(&ctx->d_blob_n, n * sizeof(int32_t)));
-    CUDA_TRY(ctx, cudaMalloc(&ctx->d_img_flags, n * sizeof(int32_t)));
-    CUDA_TRY(ctx, cudaMemsetAsync(ctx->d_seg_count, 0, n * sizeof(uint32_t), ctx->stream));   // kept zero by k_blob_reduce afterwards
-    ctx->cap_images = n_images;
-    return MOCAP_OK;
+    int st = grow_carved(ctx, ctx->images, Drain::stream, [&](Layout& L) {
+        ctx->d_seg_count = L.take<uint32_t>(n); ctx->d_work_count = L.take<uint32_t>(4);     // kept zero by the kernels afterwards
+        ctx->d_img_done = L.take<uint32_t>(n); ctx->d_set_done = L.take<uint32_t>(2 * n);
+        L.zero_so_far();
+        ctx->d_seg_list = L.take<uint32_t>(n * ctx->cfg.max_segments); ctx->d_worklist = L.take<uint32_t>(n);
+        ctx->d_set_worklist = L.take<uint32_t>(n); ctx->d_unit_counter = L.take<unsigned long long>(1);
+        ctx->d_blob_xy = L.take<int32_t>(n * ctx->cfg.max_blobs * 2); ctx->d_blob_n = L.take<int32_t>(n); ctx->d_img_flags = L.take<int32_t>(n);
+    });
+    ctx->cap_images = st ? 0 : n_images;
+    return st;
 }
 
 static int ensure_sets(mocap_ctx* ctx, int n_sets) {
     if (n_sets <= ctx->cap_sets) return MOCAP_OK;
-    CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-    cudaFree(ctx->d_obj); cudaFree(ctx->d_err); cudaFree(ctx->d_nobj); cudaFree(ctx->d_setflags);
-    ctx->d_obj = nullptr; ctx->d_err = nullptr; ctx->d_nobj = nullptr; ctx->d_setflags = nullptr; ctx->cap_sets = 0;
     const size_t n = (size_t)n_sets, R = ctx->cfg.max_roots;
-    CUDA_TRY(ctx, cudaMalloc(&ctx->d_obj, n * R * 3 * sizeof(double)));
-    CUDA_TRY(ctx, cudaMalloc(&ctx->d_err, n * R * sizeof(double)));
-    CUDA_TRY(ctx, cudaMalloc(&ctx->d_nobj, n * sizeof(int32_t)));
-    CUDA_TRY(ctx, cudaMalloc(&ctx->d_setflags, n * sizeof(int32_t)));
-    ctx->cap_sets = n_sets;
-    return MOCAP_OK;
+    int st = grow_carved(ctx, ctx->sets, Drain::stream, [&](Layout& L) {
+        ctx->d_obj = L.take<double>(n * R * 3); ctx->d_err = L.take<double>(n * R);
+        ctx->d_nobj = L.take<int32_t>(n); ctx->d_setflags = L.take<int32_t>(n);
+    });
+    ctx->cap_sets = st ? 0 : n_sets;
+    return st;
 }
 
 extern "C" {
@@ -125,13 +100,13 @@ int mocap_create(mocap_ctx** out, const mocap_config* cfg) {
 
     mocap_ctx* ctx = new (std::nothrow) mocap_ctx();
     if (!ctx) return MOCAP_ENOMEM;
-    memset(ctx, 0, sizeof(*ctx));
     ctx->cfg = *cfg;
     ctx->num_sms = prop.multiProcessorCount;
     ctx->h_tables.n_cam = cfg->n_cam;
     int st = MOCAP_OK;
     do {
-        if (cudaMalloc(&ctx->d_tables, sizeof(CameraTables)) != cudaSuccess) { st = MOCAP_ENOMEM; break; }
+        if (ctx->tables.grow(ctx, sizeof(CameraTables), Drain::none) != MOCAP_OK) { st = MOCAP_ENOMEM; break; }
+        ctx->d_tables = ctx->tables.as<CameraTables>();
         if (cudaStreamCreateWithFlags(&ctx->copy_stream, cudaStreamNonBlocking) != cudaSuccess) { st = MOCAP_ECUDA; break; }
         if (cudaStreamCreateWithFlags(&ctx->copy_stream2, cudaStreamNonBlocking) != cudaSuccess) { st = MOCAP_ECUDA; break; }
         for (int k = 0; k < 2 * 64; ++k)
@@ -152,15 +127,11 @@ int mocap_create(mocap_ctx** out, const mocap_config* cfg) {
             ctx->pipeline_auto = (mode && mode[0]) ? 0 : 1;
         }
         {
-            void* h = nullptr;
-            if (cudaHostAlloc(&h, 2 * sizeof(unsigned long long), cudaHostAllocMapped) != cudaSuccess) { st = MOCAP_ENOMEM; break; }
-            memset(h, 0, 2 * sizeof(unsigned long long));
-            ctx->h_stat = static_cast<volatile unsigned long long*>(h);
+            if (ctx->stat_host.grow(ctx, 16, Drain::none, 16, cudaHostAllocMapped) != MOCAP_OK) { st = MOCAP_ENOMEM; break; }
             void* d = nullptr;
-            if (cudaHostGetDevicePointer(&d, h, 0) != cudaSuccess) { st = MOCAP_ECUDA; break; }
+            if (cudaHostGetDevicePointer(&d, ctx->stat_host.get(), 0) != cudaSuccess) { st = MOCAP_ECUDA; break; }
             ctx->d_stat_host = static_cast<unsigned long long*>(d);
-            if (cudaMalloc(&ctx->d_stat_acc, sizeof(unsigned long long)) != cudaSuccess) { st = MOCAP_ENOMEM; break; }
-            if (cudaMemset(ctx->d_stat_acc, 0, sizeof(unsigned long long)) != cudaSuccess) { st = MOCAP_ECUDA; break; }
+            if (ctx->stat_acc.grow(ctx, 8, Drain::none, 8) != MOCAP_OK) { st = MOCAP_ENOMEM; break; }
         }
         if ((st = fused_kernel_init(ctx)) != MOCAP_OK) break;
         if ((st = ba_dev_init(ctx)) != MOCAP_OK) break;
@@ -174,25 +145,6 @@ void mocap_destroy(mocap_ctx* ctx) {
     if (!ctx) return;
     cudaSetDevice(ctx->cfg.device);
     cudaDeviceSynchronize();
-    cudaFree(ctx->d_tables);
-    cudaFree(ctx->d_seg_count); cudaFree(ctx->d_seg_list); cudaFree(ctx->d_worklist); cudaFree(ctx->d_work_count);
-    cudaFree(ctx->d_set_worklist); cudaFree(ctx->d_img_done); cudaFree(ctx->d_set_done); cudaFree(ctx->d_unit_counter);
-    cudaFree(ctx->d_blob_xy); cudaFree(ctx->d_blob_n); cudaFree(ctx->d_img_flags);
-    cudaFree(ctx->d_hole_win);
-    cudaFree(ctx->d_stage[0]); cudaFree(ctx->d_stage[1]);
-    cudaFree(ctx->d_obj); cudaFree(ctx->d_err); cudaFree(ctx->d_nobj); cudaFree(ctx->d_setflags);
-    cudaFree(ctx->d_scratch);
-    cudaFree(ctx->d_ba_ws);
-    cudaFree(ctx->d_match_counter);
-    cudaFree(ctx->d_match_items); cudaFree(ctx->d_match_partial); cudaFree(ctx->d_match_range); cudaFree(ctx->d_match_arrive);
-    cudaFree(ctx->d_pp_m1); cudaFree(ctx->d_pp_m2); cudaFree(ctx->d_pp_rot);
-    cudaFree(ctx->d_live_in); cudaFree(ctx->d_live_out);
-    cudaFree(ctx->d_palette); cudaFree(ctx->d_line_counter); cudaFree(ctx->d_line_counts);
-    if (ctx->h_live_in) cudaFreeHost(ctx->h_live_in);
-    if (ctx->h_live_out) cudaFreeHost(ctx->h_live_out);
-    jpeg_release(ctx);
-    cudaFree(ctx->d_stat_acc);
-    if (ctx->h_stat) cudaFreeHost(const_cast<unsigned long long*>(ctx->h_stat));
     if (ctx->copy_stream) cudaStreamDestroy(ctx->copy_stream);
     if (ctx->copy_stream2) cudaStreamDestroy(ctx->copy_stream2);
     for (int k = 0; k < 2 * 64; ++k) if (ctx->tim_ev[k]) cudaEventDestroy(ctx->tim_ev[k]);
@@ -246,7 +198,8 @@ int mocap_set_world_transform(mocap_ctx* ctx, const double* M) {
 static bool pick_fused(const mocap_ctx* ctx) {
     if (!ctx->use_fused) return false;
     if (!ctx->pipeline_auto) return true;
-    const unsigned long long blobs = ctx->h_stat[0], images = ctx->h_stat[1];
+    const volatile unsigned long long* h_stat = ctx->stat_host.as<volatile unsigned long long>();
+    const unsigned long long blobs = h_stat[0], images = h_stat[1];
     if (images == 0) return true;
     return (double)blobs * ctx->cfg.n_cam <= (double)MOCAP_HEAVY_BLOBS_PER_SET * (double)images;
 }
@@ -332,14 +285,11 @@ int mocap_pipeline_host(mocap_ctx* ctx, const uint8_t* frames, int n_frame_sets,
     if (chunk < 1) chunk = 1;
     if (chunk > n_frame_sets) chunk = n_frame_sets > 0 ? n_frame_sets : 1;
     const size_t need = (size_t)chunk * set_bytes;
-    if (need > ctx->stage_bytes) {
-        CUDA_TRY(ctx, cudaDeviceSynchronize());
-        for (int k = 0; k < 2; ++k) { cudaFree(ctx->d_stage[k]); ctx->d_stage[k] = nullptr; }
-        ctx->stage_bytes = 0;
-        for (int k = 0; k < 2; ++k) CUDA_TRY(ctx, cudaMalloc(&ctx->d_stage[k], need));
-        ctx->stage_bytes = need;
-    }
-    int st = ensure_sets(ctx, n_frame_sets);
+    int st = grow_carved(ctx, ctx->stage, Drain::device, [&](Layout& L) {   // the copy streams use them too
+        for (int k = 0; k < 2; ++k) ctx->d_stage[k] = L.take<uint8_t>(need);
+    });
+    if (st) return st;
+    st = ensure_sets(ctx, n_frame_sets);
     if (st) return st;
     st = ensure_images(ctx, chunk * C);
     if (st) return st;
@@ -413,16 +363,13 @@ static int tri_host_common(mocap_ctx* ctx, const double* obs, const uint8_t* mas
     const int C = ctx->cfg.n_cam;
     const size_t n = (size_t)n_points;
     const size_t b_obs = n * C * 2 * sizeof(double), b_X = n * 3 * sizeof(double), b_err = n * sizeof(double);
-    const size_t b_mask = (n * C + 15) & ~(size_t)15, b_valid = (n + 15) & ~(size_t)15;
-    int st = ensure_scratch(ctx, b_obs + 2 * b_X + b_err + b_mask + b_valid);
+    double *d_obs, *d_X, *d_Xin, *d_err;
+    uint8_t *d_mask, *d_valid;
+    int st = grow_carved(ctx, ctx->scratch, Drain::stream, [&](Layout& L) {
+        d_obs = L.take<double>(n * C * 2); d_X = L.take<double>(n * 3); d_Xin = L.take<double>(n * 3);
+        d_err = L.take<double>(n); d_mask = L.take<uint8_t>(n * C); d_valid = L.take<uint8_t>(n);
+    });
     if (st) return st;
-    unsigned char* p = static_cast<unsigned char*>(ctx->d_scratch);
-    double* d_obs = reinterpret_cast<double*>(p); p += b_obs;
-    double* d_X = reinterpret_cast<double*>(p); p += b_X;
-    double* d_Xin = reinterpret_cast<double*>(p); p += b_X;
-    double* d_err = reinterpret_cast<double*>(p); p += b_err;
-    uint8_t* d_mask = p; p += b_mask;
-    uint8_t* d_valid = p;
     CUDA_TRY(ctx, cudaMemcpyAsync(d_obs, obs, b_obs, cudaMemcpyHostToDevice, ctx->stream));
     CUDA_TRY(ctx, cudaMemcpyAsync(d_mask, mask, n * C, cudaMemcpyHostToDevice, ctx->stream));
     if (X_in) CUDA_TRY(ctx, cudaMemcpyAsync(d_Xin, X_in, b_X, cudaMemcpyHostToDevice, ctx->stream));

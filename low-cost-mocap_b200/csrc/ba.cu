@@ -603,25 +603,16 @@ int setup_problem(mocap_ctx* ctx, DeviceBA& P, const double* obs, const uint8_t*
         valid[f] = nv > 1;                                      // helpers.py:207-208,222-223: <= 1 view is skipped
         P.n_valid += valid[f];
     }
-    auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
     const size_t ncol = (size_t)n + 1;
-    const size_t sz[] = {
-        al((size_t)m * C * 2 * 8), al((size_t)m * C), al((size_t)m), al((size_t)C * 12 * 8), al(ncol * sizeof(BAColumn)), al(ncol * 8),
-        al(ncol * m * 4), al(ncol * m * 8), al((size_t)(n > 0 ? n : 1) * m * 8), al((size_t)m * 8), al((size_t)m * 8),
-        al(((size_t)n * n + 2 * n + 8) * 8), al(256), al((size_t)m * 3 * 8), al((size_t)m * 3 * 8), al((size_t)(n + 1) * 8),
-        al(((size_t)n * n + 2 * n + 8) * 8)};
-    size_t total = 0;
-    for (size_t b : sz) total += b;
-    int st = ensure_scratch(ctx, total);
+    int st = grow_carved(ctx, ctx->scratch, Drain::stream, [&](Layout& L) {
+        P.d_obs = L.take<double>((size_t)m * C * 2); P.d_mask = L.take<uint8_t>((size_t)m * C); P.d_valid = L.take<uint8_t>(m);
+        P.d_baseRt = L.take<double>((size_t)C * 12); P.d_cols = L.take<BAColumn>(ncol); P.d_dx = L.take<double>(ncol);
+        P.d_f32 = L.take<float>(ncol * m); P.d_f64 = L.take<double>(ncol * m); P.d_Js = L.take<double>((size_t)(n > 0 ? n : 1) * m);
+        P.d_fs = L.take<double>(m); P.d_cterm = L.take<double>(m); P.d_out = L.take<double>((size_t)n * n + 2 * n + 8);
+        P.d_flag = L.take<int>(64); P.d_X = L.take<double>((size_t)m * 3); P.d_Xnew = L.take<double>((size_t)m * 3);
+        P.d_dc = L.take<double>((size_t)n + 1); P.d_sba = L.take<double>((size_t)n * n + 2 * n + 8);
+    });
     if (st) return st;
-    unsigned char* p = static_cast<unsigned char*>(ctx->d_scratch);
-    int i = 0;
-    P.d_obs = (double*)p; p += sz[i++]; P.d_mask = p; p += sz[i++]; P.d_valid = p; p += sz[i++];
-    P.d_baseRt = (double*)p; p += sz[i++]; P.d_cols = (BAColumn*)p; p += sz[i++]; P.d_dx = (double*)p; p += sz[i++];
-    P.d_f32 = (float*)p; p += sz[i++]; P.d_f64 = (double*)p; p += sz[i++]; P.d_Js = (double*)p; p += sz[i++];
-    P.d_fs = (double*)p; p += sz[i++]; P.d_cterm = (double*)p; p += sz[i++]; P.d_out = (double*)p; p += sz[i++];
-    P.d_flag = (int*)p; p += sz[i++]; P.d_X = (double*)p; p += sz[i++]; P.d_Xnew = (double*)p; p += sz[i++];
-    P.d_dc = (double*)p; p += sz[i++]; P.d_sba = (double*)p; p += sz[i++];
     cudaStream_t s = ctx->stream;
     CUDA_TRY(ctx, cudaMemcpyAsync(P.d_obs, obs, (size_t)m * C * 2 * 8, cudaMemcpyHostToDevice, s));
     CUDA_TRY(ctx, cudaMemcpyAsync(P.d_mask, mask, (size_t)m * C, cudaMemcpyHostToDevice, s));
@@ -694,14 +685,14 @@ int mocap_bundle_adjust_host(mocap_ctx* ctx, const double* obs, const uint8_t* m
     if (opt.engine == 0) {
         // default: copy in, ONE launch of the device-resident solve (mocap_bundle_adjust_dev), copy out
         const int C = ctx->cfg.n_cam;
-        auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
-        const size_t b_obs = al((size_t)n_points * C * 2 * 8), b_mask = al((size_t)n_points * C), b_R = al((size_t)C * 9 * 8), b_t = al((size_t)C * 3 * 8);
-        int st = ensure_scratch(ctx, b_obs + b_mask + b_R + b_t + al(sizeof(mocap_ba_report)));
+        double *d_obs, *d_R, *d_t;
+        uint8_t* d_mask;
+        mocap_ba_report* d_rep;
+        int st = grow_carved(ctx, ctx->scratch, Drain::stream, [&](Layout& L) {
+            d_obs = L.take<double>((size_t)n_points * C * 2); d_mask = L.take<uint8_t>((size_t)n_points * C);
+            d_R = L.take<double>((size_t)C * 9); d_t = L.take<double>((size_t)C * 3); d_rep = L.take<mocap_ba_report>(1);
+        });
         if (st) return st;
-        unsigned char* p = static_cast<unsigned char*>(ctx->d_scratch);
-        double* d_obs = (double*)p; p += b_obs; uint8_t* d_mask = p; p += b_mask;
-        double* d_R = (double*)p; p += b_R; double* d_t = (double*)p; p += b_t;
-        mocap_ba_report* d_rep = (mocap_ba_report*)p;
         cudaStream_t s = ctx->stream;
         CUDA_TRY(ctx, cudaMemcpyAsync(d_obs, obs, (size_t)n_points * C * 2 * 8, cudaMemcpyHostToDevice, s));
         CUDA_TRY(ctx, cudaMemcpyAsync(d_mask, mask, (size_t)n_points * C, cudaMemcpyHostToDevice, s));

@@ -118,35 +118,23 @@ struct BAWorkspace {
 static int ba_workspace(mocap_ctx* ctx, int K, const int* m_max, const int* g, int n_sets, BAWorkspace& W, int* pstride_out) {
     const int C = ctx->cfg.n_cam, n = 6 * (C - 1), npair = n * (n + 1) / 2;
     const int pstride = npair + 2 * n + 8;
-    auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
-    auto problem_bytes = [&](int m, int G) {
-        return al((size_t)m * 3 * 8) + al((size_t)m * 3 * 8) + al((size_t)m) + al((size_t)G * pstride * 8) + al((size_t)pstride * 8) +
-               al((size_t)2 * G * 4 * 8);
-    };
-    const size_t bar_bytes = al((size_t)MOCAP_BA_MAX_BATCH * BA_BAR_LINE);
-    size_t total = bar_bytes + al((size_t)C * 12 * 8) + al((size_t)(n_sets > 0 ? n_sets : 1) * 4) + al(sizeof(mocap_ba_report));
-    for (int k = 0; k < K; ++k) total += problem_bytes(m_max[k], g[k]);
-    if (total > ctx->ba_ws_bytes) {
-        CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-        cudaFree(ctx->d_ba_ws);
-        ctx->d_ba_ws = nullptr; ctx->ba_ws_bytes = 0;
-        CUDA_TRY(ctx, cudaMalloc(&ctx->d_ba_ws, total));
-        ctx->ba_ws_bytes = total;
-        CUDA_TRY(ctx, cudaMemsetAsync(ctx->d_ba_ws, 0, total, ctx->stream));     // the grid barriers start at zero
-    }
-    unsigned char* p = static_cast<unsigned char*>(ctx->d_ba_ws);
-    // the barrier words come FIRST so that they keep their place (and their generation counts) when nothing grows
-    unsigned char* bars = p; p += bar_bytes;
-    for (int k = 0; k < K; ++k) {
-        BAProblemWS& w = W.pr[k];
-        const size_t m = (size_t)m_max[k], G = (size_t)g[k];
-        w.bar = (unsigned*)(bars + (size_t)k * BA_BAR_LINE);
-        w.X = (double*)p; p += al(m * 3 * 8); w.Xnew = (double*)p; p += al(m * 3 * 8); w.valid = p; p += al(m);
-        w.part = (double*)p; p += al(G * pstride * 8); w.fin = (double*)p; p += al((size_t)pstride * 8);
-        w.cpart = (double*)p; p += al(2 * G * 4 * 8);
-    }
-    W.Rt_io = (double*)p; p += al((size_t)C * 12 * 8); W.offs = (int32_t*)p; p += al((size_t)(n_sets > 0 ? n_sets : 1) * 4);
-    W.report = (mocap_ba_report*)p;
+    const size_t sets = n_sets > 0 ? n_sets : 1;
+    // the whole workspace is zeroed when it grows (the grid barriers start at zero); the barrier words come FIRST so
+    // that they keep their place (and their generation counts) when nothing grows
+    int st = grow_carved(ctx, ctx->ba_ws, Drain::stream, [&](Layout& L) {
+        uint8_t* bars = L.take<uint8_t>((size_t)MOCAP_BA_MAX_BATCH * BA_BAR_LINE);
+        for (int k = 0; k < K; ++k) {
+            BAProblemWS& w = W.pr[k];
+            const size_t m = (size_t)m_max[k], G = (size_t)g[k];
+            w.bar = bars ? (unsigned*)(bars + (size_t)k * BA_BAR_LINE) : nullptr;
+            w.X = L.take<double>(m * 3); w.Xnew = L.take<double>(m * 3); w.valid = L.take<uint8_t>(m);
+            w.part = L.take<double>(G * pstride); w.fin = L.take<double>(pstride); w.cpart = L.take<double>(2 * G * 4);
+        }
+        W.Rt_io = L.take<double>((size_t)C * 12); W.offs = L.take<int32_t>(sets);
+        W.report = L.take<mocap_ba_report>(1);
+        L.zero_so_far();
+    });
+    if (st) return st;
     *pstride_out = pstride;
     return MOCAP_OK;
 }

@@ -277,14 +277,14 @@ int launch_blob_fallback(mocap_ctx* ctx, int32_t* blob_xy, int32_t* blob_n, int6
         k_blob_reduce<NT, true><<<grid2, NT, smem, ctx->stream>>>(ctx->d_seg_count, ctx->d_seg_list, E, c.width, c.height,
                                                                c.max_blobs, blob_xy, blob_n, blob_mom, img_flags,
                                                                ctx->d_worklist, ctx->d_work_count, ctx->d_work_count + 1,
-                                                               n_images, ctx->d_stat_acc, ctx->pipeline_auto ? ctx->d_stat_host : nullptr,
-                                                               ctx->d_hole_win);
+                                                               n_images, ctx->stat_acc.as<unsigned long long>(), ctx->pipeline_auto ? ctx->d_stat_host : nullptr,
+                                                               ctx->hole_win.as<unsigned long long>());
     else
         k_blob_reduce<NT, false><<<grid2, NT, smem, ctx->stream>>>(ctx->d_seg_count, ctx->d_seg_list, E, c.width, c.height,
                                                                 c.max_blobs, blob_xy, blob_n, blob_mom, img_flags,
                                                                 ctx->d_worklist, ctx->d_work_count, ctx->d_work_count + 1,
-                                                               n_images, ctx->d_stat_acc, ctx->pipeline_auto ? ctx->d_stat_host : nullptr,
-                                                               ctx->d_hole_win);
+                                                               n_images, ctx->stat_acc.as<unsigned long long>(), ctx->pipeline_auto ? ctx->d_stat_host : nullptr,
+                                                               ctx->hole_win.as<unsigned long long>());
     CUDA_TRY(ctx, cudaGetLastError());
     ctx->launches += 1;
     return MOCAP_OK;
@@ -304,19 +304,15 @@ int timing_flush(mocap_ctx* ctx) {
 
 // the whole-image window of the RETR_TREE slow path, one per CTA of k_blob_reduce (grid = num_sms): on = allocate, off = free
 int blob_set_large_holes(mocap_ctx* ctx, int on) {
-    if (!on == !ctx->d_hole_win) return MOCAP_OK;
+    if (!on == !ctx->hole_win.get()) return MOCAP_OK;
     CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));          // a k_blob_reduce in flight may still use the scratch
     if (!on) {
-        CUDA_TRY(ctx, cudaFree(ctx->d_hole_win));
-        ctx->d_hole_win = nullptr;
+        ctx->hole_win.reset();
         return MOCAP_OK;
     }
     const size_t bytes = (size_t)ctx->num_sms * 4 * hole_wide_words(ctx->cfg.width, ctx->cfg.height) * sizeof(unsigned long long);
-    if (cudaMalloc(&ctx->d_hole_win, bytes) != cudaSuccess) {
-        cudaGetLastError();
-        ctx->d_hole_win = nullptr;
+    if (ctx->hole_win.grow(ctx, bytes, Drain::none) != MOCAP_OK)
         return mocap_fail(ctx, MOCAP_ENOMEM, "mocap_set_large_holes: %zu bytes of device memory for the whole-image windows", bytes);
-    }
     return MOCAP_OK;
 }
 

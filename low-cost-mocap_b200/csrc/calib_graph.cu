@@ -248,8 +248,6 @@ k_translation_residuals(const double* __restrict__ obs, const uint8_t* __restric
     front[idx] = fr;
 }
 
-static size_t a256(size_t b) { return (b + 255) & ~(size_t)255; }
-
 static void hartley(const std::vector<float4>& pts, int o, int m, const std::vector<uint8_t>& inl, double T[6]) {
     for (int side = 0; side < 2; ++side) {
         double cx = 0, cy = 0; int k = 0;
@@ -373,33 +371,17 @@ extern "C" int mocap_calibrate_graph_host(mocap_ctx* ctx, const double* obs, con
     const int n3 = 3 * C, E = n3 * (n3 + 1) / 2;
     const int chunk = 64;
     const int G = (n_points + chunk - 1) / chunk;
-    const size_t b_pts = a256(total * sizeof(float4)), b_off = a256((P + 1) * sizeof(int)), b_inl = a256(total);
-    const size_t b_T = a256((size_t)P * 6 * 8), b_45 = a256((size_t)P * 45 * 8), b_F = a256((size_t)P * 9 * 8);
-    const size_t b_cand = a256((size_t)P * 4 * CG_CAND * 8), b_cnt = a256((size_t)P * 4 * sizeof(int)), b_ang = a256(total * 4 * 8);
-    const size_t b_obs = a256(nv * 2 * 8), b_init = a256(nv), b_w = a256(nv * 8), b_front = a256(nv), b_cams = a256(sizeof(CgCams));
-    const size_t b_t = a256(n3 * 8), b_part = a256((size_t)G * E * 8), b_H = a256((size_t)E * 8);
-    st = ensure_scratch(ctx, b_pts + b_off + b_inl + b_T + b_45 + b_F + b_cand + b_cnt + b_ang + b_obs + b_init + 2 * b_w + b_front + b_cams +
-                                 b_t + b_part + b_H);
+    float4* d_pts; int *d_off, *d_cnt; uint8_t *d_inl, *d_init, *d_front; CgCams* d_cams;
+    double *d_T, *d_45, *d_F, *d_cand, *d_ang, *d_obs, *d_w[2], *d_t, *d_part, *d_H;
+    st = grow_carved(ctx, ctx->scratch, Drain::stream, [&](Layout& L) {
+        d_pts = L.take<float4>(total); d_off = L.take<int>(P + 1); d_inl = L.take<uint8_t>(total);
+        d_T = L.take<double>((size_t)P * 6); d_45 = L.take<double>((size_t)P * 45); d_F = L.take<double>((size_t)P * 9);
+        d_cand = L.take<double>((size_t)P * 4 * CG_CAND); d_cnt = L.take<int>((size_t)P * 4); d_ang = L.take<double>(total * 4);
+        d_obs = L.take<double>(nv * 2); d_init = L.take<uint8_t>(nv); d_w[0] = L.take<double>(nv); d_w[1] = L.take<double>(nv);
+        d_front = L.take<uint8_t>(nv); d_cams = L.take<CgCams>(1);
+        d_t = L.take<double>(n3); d_part = L.take<double>((size_t)G * E); d_H = L.take<double>(E);
+    });
     if (st) { cudaGetLastError(); return st; }
-    unsigned char* base = static_cast<unsigned char*>(ctx->d_scratch);
-    auto take = [&](size_t bytes) { unsigned char* q = base; base += bytes; return q; };
-    float4* d_pts = reinterpret_cast<float4*>(take(b_pts));
-    int* d_off = reinterpret_cast<int*>(take(b_off));
-    uint8_t* d_inl = take(b_inl);
-    double* d_T = reinterpret_cast<double*>(take(b_T));
-    double* d_45 = reinterpret_cast<double*>(take(b_45));
-    double* d_F = reinterpret_cast<double*>(take(b_F));
-    double* d_cand = reinterpret_cast<double*>(take(b_cand));
-    int* d_cnt = reinterpret_cast<int*>(take(b_cnt));
-    double* d_ang = reinterpret_cast<double*>(take(b_ang));
-    double* d_obs = reinterpret_cast<double*>(take(b_obs));
-    uint8_t* d_init = take(b_init);
-    double* d_w[2] = {reinterpret_cast<double*>(take(b_w)), reinterpret_cast<double*>(take(b_w))};
-    uint8_t* d_front = take(b_front);
-    CgCams* d_cams = reinterpret_cast<CgCams*>(take(b_cams));
-    double* d_t = reinterpret_cast<double*>(take(b_t));
-    double* d_part = reinterpret_cast<double*>(take(b_part));
-    double* d_H = reinterpret_cast<double*>(take(b_H));
     cudaStream_t s = ctx->stream;
     CUDA_TRY(ctx, cudaMemcpyAsync(d_pts, pts.data(), total * sizeof(float4), cudaMemcpyHostToDevice, s));
     CUDA_TRY(ctx, cudaMemcpyAsync(d_off, off.data(), (P + 1) * sizeof(int), cudaMemcpyHostToDevice, s));

@@ -218,13 +218,14 @@ int calibrate_chain(mocap_ctx* ctx, const double* obs, const uint8_t* mask, int 
     const int C = ctx->cfg.n_cam;
     CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));
     const size_t n = (size_t)n_points;
-    int st = ensure_scratch(ctx, n * 2 * 8 * 2 + n + 4096);
+    double *d_p1, *d_p2, *d_work;
+    uint8_t* d_inl;
+    int st = grow_carved(ctx, ctx->scratch, Drain::stream, [&](Layout& L) {
+        d_p1 = L.take<double>(2 * n); d_p2 = L.take<double>(2 * n);
+        d_work = L.take<double>(256);                // small device scratch of pair_motion
+        d_inl = L.take<uint8_t>(n);
+    });
     if (st) return st;
-    unsigned char* base = static_cast<unsigned char*>(ctx->d_scratch);
-    double* d_p1 = reinterpret_cast<double*>(base);
-    double* d_p2 = d_p1 + 2 * n;
-    double* d_work = d_p2 + 2 * n;                 // 256 doubles of small device scratch
-    uint8_t* d_inl = reinterpret_cast<uint8_t*>(d_work + 256);
     // camera 0: (I, 0)   (index.py:235-238)
     for (int i = 0; i < 9; ++i) R[i] = (i % 4 == 0) ? 1.0 : 0.0;
     t[0] = t[1] = t[2] = 0.0;

@@ -89,8 +89,6 @@ k_ransac_mask(const float4* __restrict__ pts, const int* __restrict__ off, int H
     }
 }
 
-static size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
-
 int ransac_check_options(mocap_ctx* ctx, const mocap_ransac_options* opt, mocap_ransac_options* o, const char* who) {
     mocap_ransac_default_options(o);
     if (opt) *o = *opt;
@@ -100,31 +98,19 @@ int ransac_check_options(mocap_ctx* ctx, const mocap_ransac_options* opt, mocap_
     return MOCAP_OK;
 }
 
-size_t ransac_scratch_bytes(int P, size_t total, int H) {
-    return align256(total * sizeof(float4)) + align256((P + 1) * sizeof(int)) + align256((size_t)P * H * 27 * sizeof(double)) +
-           align256((size_t)P * H * sizeof(int)) + align256(P * sizeof(unsigned long long)) + align256(P * 9 * sizeof(double)) +
-           align256(total);
-}
-
 int ransac_run(mocap_ctx* ctx, const float4* h_pts, const int* h_off, int P, const mocap_ransac_options& o, double* F_best,
                uint8_t* inl, unsigned long long* keys) {
     const int H = o.hypotheses;
     const double thr2 = o.threshold_px * o.threshold_px;
     const size_t total = (size_t)h_off[P];
     CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));
-    const size_t b_pts = align256(total * sizeof(float4)), b_off = align256((P + 1) * sizeof(int));
-    const size_t b_models = align256((size_t)P * H * 27 * sizeof(double)), b_n = align256((size_t)P * H * sizeof(int));
-    const size_t b_best = align256(P * sizeof(unsigned long long)), b_F = align256(P * 9 * sizeof(double));
-    int st = ensure_scratch(ctx, ransac_scratch_bytes(P, total, H));
+    float4* d_pts; int *d_off, *d_n; double *d_models, *d_F; unsigned long long* d_best; uint8_t* d_inl;
+    int st = grow_carved(ctx, ctx->scratch, Drain::stream, [&](Layout& L) {
+        d_pts = L.take<float4>(total); d_off = L.take<int>(P + 1);
+        d_models = L.take<double>((size_t)P * H * 27); d_n = L.take<int>((size_t)P * H);
+        d_best = L.take<unsigned long long>(P); d_F = L.take<double>((size_t)P * 9); d_inl = L.take<uint8_t>(total);
+    });
     if (st) return st;
-    unsigned char* b = static_cast<unsigned char*>(ctx->d_scratch);
-    float4* d_pts = reinterpret_cast<float4*>(b); b += b_pts;
-    int* d_off = reinterpret_cast<int*>(b); b += b_off;
-    double* d_models = reinterpret_cast<double*>(b); b += b_models;
-    int* d_n = reinterpret_cast<int*>(b); b += b_n;
-    unsigned long long* d_best = reinterpret_cast<unsigned long long*>(b); b += b_best;
-    double* d_F = reinterpret_cast<double*>(b); b += b_F;
-    uint8_t* d_inl = b;
     cudaStream_t s = ctx->stream;
     CUDA_TRY(ctx, cudaMemcpyAsync(d_pts, h_pts, total * sizeof(float4), cudaMemcpyHostToDevice, s));
     CUDA_TRY(ctx, cudaMemcpyAsync(d_off, h_off, (P + 1) * sizeof(int), cudaMemcpyHostToDevice, s));

@@ -5,6 +5,7 @@
 #include <stdio.h>
 #include <string.h>
 #include "../../include/mocap_b200.h"
+#include "ctx_memory.h"
 
 #define MOCAP_MAX_CAM        16
 #define MOCAP_MAX_BLOBS      64
@@ -33,59 +34,64 @@ struct mocap_ctx {
     cudaStream_t copy_stream2;   // staging buffers alternate between two copy streams (two copy engines in flight)
     char         err[512];
     bool         cameras_set;
-    CameraTables* d_tables;
+    DeviceBuffer  tables; CameraTables* d_tables;      // d_tables = tables
     CameraTables  h_tables;
-    // detection scratch, sized for cap_images
+    // detection scratch, sized for cap_images; the first four regions are self-resetting counters, zeroed when it grows
+    DeviceBuffer images;
     int       cap_images;
     uint32_t* d_seg_count;
-    uint32_t* d_seg_list;
-    uint32_t* d_worklist;     // images deferred by the warp-level blob kernel
     uint32_t* d_work_count;   // [4]: image worklist count + finished-CTA counter, set worklist count + finished-CTA counter
-    uint32_t* d_set_worklist; // frame-sets deferred by the fused kernel
     uint32_t* d_img_done;     // fused kernel: finished units per image (self-resetting)
     uint32_t* d_set_done;     // fused kernel: [2*cap_images] finished images per set, then deferred marks
+    uint32_t* d_seg_list;
+    uint32_t* d_worklist;     // images deferred by the warp-level blob kernel
+    uint32_t* d_set_worklist; // frame-sets deferred by the fused kernel
     unsigned long long* d_unit_counter;
-    int       fused_ctas_per_sm;
-    int       pipeline_auto;     // MOCAP_PIPELINE unset: heavy batches (many blobs per frame-set) take the three-kernel pipeline
-    unsigned long long* d_stat_acc;                  // device accumulator of the blob statistic
-    volatile unsigned long long* h_stat;             // pinned, mapped: {blobs, images} of the last batch, written by the GPU
-    unsigned long long* d_stat_host;                 // device alias of h_stat
-    int       use_fused;      // 1: single fused pipeline kernel for 1-channel frames (default)
-    unsigned long long* d_hole_win;   // mocap_set_large_holes: the whole-image windows of k_blob_reduce's CTAs; nullptr = off
     int32_t*  d_blob_xy;
     int32_t*  d_blob_n;
     int32_t*  d_img_flags;
+    int       fused_ctas_per_sm;
+    int       pipeline_auto;     // MOCAP_PIPELINE unset: heavy batches (many blobs per frame-set) take the three-kernel pipeline
+    DeviceBuffer stat_acc;                           // device accumulator of the blob statistic
+    PinnedBuffer stat_host;                          // mapped: {blobs, images} of the last batch, written by the GPU
+    unsigned long long* d_stat_host;                 // device alias of stat_host
+    int       use_fused;      // 1: single fused pipeline kernel for 1-channel frames (default)
+    DeviceBuffer hole_win;    // mocap_set_large_holes: the whole-image windows of k_blob_reduce's CTAs; empty = off
     int       overlay_on;       // mocap_set_overlay: the live entry points draw the detection overlay (overlay.cu)
-    uint8_t*  d_palette; int palette_len;          // the epipolar lines' colours [palette_len][3]
-    unsigned long long* d_line_counter;            // epipolar lines drawn since mocap_set_overlay
-    uint32_t* d_line_counts; int line_counts_cap;  // lines per frame-set of a launch group
-    // host-path staging
+    DeviceBuffer palette; int palette_len;         // the epipolar lines' colours [palette_len][3]
+    DeviceBuffer line_counter;                     // epipolar lines drawn since mocap_set_overlay
+    DeviceBuffer line_counts;                      // lines per frame-set of a launch group
+    // host-path staging: both buffers in one allocation
+    DeviceBuffer stage;
     uint8_t*  d_stage[2];
-    size_t    stage_bytes;
     cudaEvent_t stage_free[2]; cudaEvent_t copied[2];   // per staging buffer: its kernel has finished / its copy has landed
+    DeviceBuffer sets;
     double*   d_obj; double* d_err; int32_t* d_nobj; int32_t* d_setflags;
     int       cap_sets;
-    // generic scratch for the *_host triangulation / BA entry points
-    void*     d_scratch; size_t scratch_bytes;
+    // Generic scratch of the *_host entry points, the calibration and the grey planes of the raw-frame chain.  A
+    // function that holds pointers carved from it must not call another user of it: that call may grow it (the
+    // pointers dangle) or overwrite it.
+    DeviceBuffer scratch;
     // S4 on the device (ba_dev.cu): workspace of k_ba_solve, launch shape
-    void*     d_ba_ws; size_t ba_ws_bytes; int ba_threads; int ba_grid; size_t ba_smem;
-    unsigned* d_match_counter; int match_ctas_per_sm;   // k_match_triangulate: claim counters [4], resident CTAs per SM
-    // chunked matcher (match_device.cuh MatchSplit): items, their partial results, the roots each touches, arrivals per frame-set
-    void* d_match_items; unsigned long long* d_match_partial; int* d_match_range; unsigned* d_match_arrive;
+    DeviceBuffer ba_ws; int ba_threads; int ba_grid; size_t ba_smem;
+    DeviceBuffer match_counter; int match_ctas_per_sm;  // k_match_triangulate: claim counters [4], resident CTAs per SM
+    // chunked matcher (match_device.cuh MatchSplit): arrivals per frame-set (zeroed when it grows), items, their partial
+    // results, the roots each touches
+    DeviceBuffer match_split;
+    unsigned* d_match_arrive; void* d_match_items; unsigned long long* d_match_partial; int* d_match_range;
     int match_chunk, match_item_cap, match_cap_sets;
     const int32_t* img_flags_cur;   // set by the pipelines: the matcher folds the images' S1 flags into the frame-set's
     int32_t*  track_xy_cur;   // set for the duration of mocap_pipeline_tracks_dev: where the matcher leaves the winners' pixels
-    // capture-side preprocessing (SURVEY 8(f) #2)
-    int16_t*  d_pp_m1; uint16_t* d_pp_m2; int* d_pp_rot; int pp_in_w, pp_in_h;
+    // capture-side preprocessing (SURVEY 8(f) #2); pp_in_w != 0 once mocap_set_preprocess has put all three maps on the device
+    DeviceBuffer pp_m1, pp_m2, pp_rot; int pp_in_w, pp_in_h;
     // mocap_live_host staging: device and page-locked host buffers of {timestamps, raw frames} and {result, frames}
-    uint8_t*  d_live_in; uint8_t* h_live_in; size_t live_in_bytes;
-    uint8_t*  d_live_out; uint8_t* h_live_out; size_t live_out_bytes;
+    DeviceBuffer live_in, live_out;
+    PinnedBuffer live_in_host, live_out_host;
     // JPEG encoder (jpeg.cu): device tables + header per (width, height, quality), scratch of a group of images, and
     // mocap_live_jpeg_host's device output and page-locked staging
-    uint8_t*  jpeg_cfg[16]; int jpeg_cfg_key[16][3]; int jpeg_cfg_n;
-    uint8_t*  d_jpeg_scratch; size_t jpeg_scratch_bytes;
-    uint8_t*  d_jpeg_out; size_t jpeg_out_bytes;
-    uint8_t*  h_jpeg_out; size_t jpeg_host_bytes;
+    DeviceBuffer jpeg_cfg[16]; int jpeg_cfg_key[16][3]; int jpeg_cfg_n;
+    DeviceBuffer jpeg_scratch, jpeg_out;
+    PinnedBuffer jpeg_host;
     // accounting
     uint64_t  launches;
     int       timing_on;
@@ -112,7 +118,6 @@ int launch_match(mocap_ctx* ctx, const int32_t* blob_xy, const int32_t* blob_n, 
                  double* obj, double* err, int32_t* n_obj, int32_t* set_flags, int32_t* chosen);
 int launch_triangulate(mocap_ctx* ctx, const double* obs, const uint8_t* mask, int n_points,
                        const double* X_in, double* X, double* err, uint8_t* valid);
-int ensure_scratch(mocap_ctx* ctx, size_t bytes);
 int ensure_images(mocap_ctx* ctx, int n_images);
 // the live loop's per-read outputs k_live_blobs writes (slices of the mocap_live_dev result, indexed by read)
 struct LiveOut {
@@ -126,10 +131,11 @@ int launch_overlay(mocap_ctx* ctx, const uint8_t* gray, uint8_t* frames, int n_i
 int launch_epilines(mocap_ctx* ctx, uint8_t* frames, int n_sets, const int32_t* blob_xy, const int32_t* blob_n);
 // mocap_live_host in two halves (live.cu), so that mocap_live_jpeg_host runs the same chain: live_check; live_host_run
 // (staging in, the chain; the frames stay on the device when keep_frames); live_host_finish (result, frames and
-// extra_bytes of device data back, one synchronisation)
+// extra_bytes of device data back, one synchronisation).  frame_off, extra_off: where the frames and the extra bytes
+// sit in the output staging (the result is at 0).
 struct LiveHostRun {
     mocap_live_offsets L;
-    size_t res_bytes, frame_bytes, frame_copy, extra_bytes;
+    size_t frame_copy, extra_bytes, frame_off, extra_off;
     uint8_t* d_frames;
 };
 int live_check(mocap_ctx* ctx, mocap_tracker* tr, const void* raw, int n_reads, int mode, const double* timestamps,
@@ -137,10 +143,9 @@ int live_check(mocap_ctx* ctx, mocap_tracker* tr, const void* raw, int n_reads, 
 int live_host_run(mocap_ctx* ctx, mocap_tracker* tr, const uint8_t* raw, int n_reads, int mode, const double* timestamps,
                   int keep_frames, size_t extra_bytes, LiveHostRun* run);
 int live_host_finish(mocap_ctx* ctx, const LiveHostRun& run, uint8_t* frames, void* result, const void* extra, void* extra_out);
-// the JPEG encoder (jpeg.cu): mocap_encode_jpeg_dev after its checks; the context's JPEG buffers freed
+// the JPEG encoder (jpeg.cu): mocap_encode_jpeg_dev after its checks
 int jpeg_encode(mocap_ctx* ctx, const uint8_t* images, int n_images, int tiles, int tile_w, int tile_h, int quality,
                 uint8_t* out, uint64_t out_stride, int32_t* out_len);
-void jpeg_release(mocap_ctx* ctx);
 #define MOCAP_JPEG_CONFIGS 16                     // (width, height, quality) configurations cached per context
 #define JPEG_CONFIG_BYTES  3200                   // JpegTables + the header, padded (jpeg.cuh)
 // raw frames -> preprocessing [-> S1 [-> S2+S3]] per launch group (preproc.cu)
@@ -172,8 +177,7 @@ int calibrate_chain(mocap_ctx* ctx, const double* obs, const uint8_t* mask, int 
 // defaults) or fails with MOCAP_EINVAL.  ransac_run: h_pts holds every pair's common observations {x_a, y_a, x_b, y_b}
 // (float32), pair p at [h_off[p], h_off[p+1]); pair p's samples are drawn from the hash of (seed, p, ...).  Out: F_best
 // [P][9], inl over h_pts, keys [P] (0: no sample of that pair gave a model).  Three launches, one synchronisation.
-// Scratch: ransac_scratch_bytes, dominated by P * hypotheses * 27 doubles of models.
+// Scratch: dominated by P * hypotheses * 27 doubles of models.
 int ransac_check_options(mocap_ctx* ctx, const mocap_ransac_options* opt, mocap_ransac_options* o, const char* who);
-size_t ransac_scratch_bytes(int P, size_t total, int H);
 int ransac_run(mocap_ctx* ctx, const float4* h_pts, const int* h_off, int P, const mocap_ransac_options& o, double* F_best,
                uint8_t* inl, unsigned long long* keys);

@@ -21,7 +21,7 @@
 
 static_assert(sizeof(JpegTables) + JPEG_HEADER_BYTES <= JPEG_CONFIG_BYTES, "JPEG_CONFIG_BYTES holds the tables and the header");
 static_assert(sizeof(JpegTables) % 4 == 0, "k_jpeg_* copy the tables to shared memory in words");
-static_assert(sizeof(((mocap_ctx*)0)->jpeg_cfg) / sizeof(uint8_t*) == MOCAP_JPEG_CONFIGS, "one cache slot per configuration");
+static_assert(sizeof(((mocap_ctx*)0)->jpeg_cfg) / sizeof(DeviceBuffer) == MOCAP_JPEG_CONFIGS, "one cache slot per configuration");
 
 struct JpegShape {
     int tiles, tile_w, tile_h, W, mw, mh, wb, hb, n_mcu;
@@ -42,7 +42,8 @@ static JpegShape jpeg_shape(int tiles, int tile_w, int tile_h) {
     return s;
 }
 
-// per image: coefficients, AC bits per block, MCU offsets (+ the total), words
+// per image: coefficients, AC bits per block, MCU offsets (+ the total), words; picks how many images share the
+// scratch (jpeg_encode's layout sizes it)
 static size_t jpeg_image_scratch(const JpegShape& s) {
     return s.coef_stride * 2 + (size_t)s.n_mcu * 6 * 2 + s.off_stride * 8 + s.word_stride * 4 + 64;
 }
@@ -202,24 +203,25 @@ k_jpeg_emit(JpegShape s, const uint8_t* __restrict__ header, const uint64_t* __r
 static int jpeg_config(mocap_ctx* ctx, int width, int height, int quality, const uint8_t** d_cfg) {
     for (int k = 0; k < ctx->jpeg_cfg_n; ++k)
         if (ctx->jpeg_cfg_key[k][0] == width && ctx->jpeg_cfg_key[k][1] == height && ctx->jpeg_cfg_key[k][2] == quality) {
-            *d_cfg = ctx->jpeg_cfg[k];
+            *d_cfg = ctx->jpeg_cfg[k].as<uint8_t>();
             return MOCAP_OK;
         }
     if (ctx->jpeg_cfg_n == MOCAP_JPEG_CONFIGS) {
         CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-        for (int k = 0; k < ctx->jpeg_cfg_n; ++k) cudaFree(ctx->jpeg_cfg[k]);
+        for (int k = 0; k < ctx->jpeg_cfg_n; ++k) ctx->jpeg_cfg[k].reset();
         ctx->jpeg_cfg_n = 0;
     }
     uint8_t host[JPEG_CONFIG_BYTES];
     memset(host, 0, sizeof host);
     jpeg_build_tables(quality, reinterpret_cast<JpegTables*>(host));
     jpeg_build_header(width, height, quality, host + sizeof(JpegTables));
-    uint8_t* d = nullptr;
-    CUDA_TRY(ctx, cudaMalloc(&d, JPEG_CONFIG_BYTES));
+    const int k = ctx->jpeg_cfg_n;
+    const int st = ctx->jpeg_cfg[k].grow(ctx, JPEG_CONFIG_BYTES, Drain::none);
+    if (st) return st;
+    uint8_t* d = ctx->jpeg_cfg[k].as<uint8_t>();
     // pageable source: the call returns once the bytes are staged, so `host` may go out of scope
     CUDA_TRY(ctx, cudaMemcpyAsync(d, host, JPEG_CONFIG_BYTES, cudaMemcpyHostToDevice, ctx->stream));
-    const int k = ctx->jpeg_cfg_n++;
-    ctx->jpeg_cfg[k] = d;
+    ctx->jpeg_cfg_n++;
     ctx->jpeg_cfg_key[k][0] = width; ctx->jpeg_cfg_key[k][1] = height; ctx->jpeg_cfg_key[k][2] = quality;
     *d_cfg = d;
     return MOCAP_OK;
@@ -248,19 +250,12 @@ int jpeg_encode(mocap_ctx* ctx, const uint8_t* images, int n_images, int tiles, 
     size_t fit = JPEG_GROUP_SCRATCH / per;
     if (fit < 1) fit = 1;
     const int group = fit < (size_t)n_images ? (int)fit : n_images;
-    const size_t need = per * group;
-    if (need > ctx->jpeg_scratch_bytes) {
-        CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-        cudaFree(ctx->d_jpeg_scratch);
-        ctx->d_jpeg_scratch = nullptr; ctx->jpeg_scratch_bytes = 0;
-        CUDA_TRY(ctx, cudaMalloc(&ctx->d_jpeg_scratch, need));
-        ctx->jpeg_scratch_bytes = need;
-    }
-    uint8_t* p = ctx->d_jpeg_scratch;
-    int16_t* coef = reinterpret_cast<int16_t*>(p);           p += (s.coef_stride * 2 * group + 15) & ~(size_t)15;
-    uint16_t* ac = reinterpret_cast<uint16_t*>(p);           p += ((size_t)s.n_mcu * 6 * 2 * group + 15) & ~(size_t)15;
-    uint64_t* offs = reinterpret_cast<uint64_t*>(p);         p += (s.off_stride * 8 * group + 15) & ~(size_t)15;
-    uint32_t* words = reinterpret_cast<uint32_t*>(p);
+    int16_t* coef; uint16_t* ac; uint64_t* offs; uint32_t* words;
+    st = grow_carved(ctx, ctx->jpeg_scratch, Drain::stream, [&](Layout& L) {
+        coef = L.take<int16_t>(s.coef_stride * group); ac = L.take<uint16_t>((size_t)s.n_mcu * 6 * group);
+        offs = L.take<uint64_t>(s.off_stride * group); words = L.take<uint32_t>(s.word_stride * group);
+    });
+    if (st) return st;
     for (int i0 = 0; i0 < n_images; i0 += group) {
         const int g = n_images - i0 < group ? n_images - i0 : group;
         const size_t nb = (size_t)s.n_mcu * 6 * g, nm = (size_t)s.n_mcu * g;
@@ -272,25 +267,6 @@ int jpeg_encode(mocap_ctx* ctx, const uint8_t* images, int n_images, int tiles, 
         CUDA_TRY(ctx, cudaGetLastError());
         ctx->launches += 4;
     }
-    return MOCAP_OK;
-}
-
-void jpeg_release(mocap_ctx* ctx) {
-    for (int k = 0; k < ctx->jpeg_cfg_n; ++k) cudaFree(ctx->jpeg_cfg[k]);
-    ctx->jpeg_cfg_n = 0;
-    cudaFree(ctx->d_jpeg_scratch);
-    cudaFree(ctx->d_jpeg_out);
-    if (ctx->h_jpeg_out) cudaFreeHost(ctx->h_jpeg_out);
-}
-
-// grows a device buffer (after the stream drains)
-static int ensure_device(mocap_ctx* ctx, uint8_t** d, size_t* have, size_t bytes) {
-    if (bytes <= *have) return MOCAP_OK;
-    CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-    cudaFree(*d);
-    *d = nullptr; *have = 0;
-    CUDA_TRY(ctx, cudaMalloc(d, bytes));
-    *have = bytes;
     return MOCAP_OK;
 }
 
@@ -322,11 +298,14 @@ int mocap_live_jpeg_host(mocap_ctx* ctx, mocap_tracker* tr, const uint8_t* raw, 
     const uint64_t bound = jpeg_bound(C * S, S);
     // rows of the device output: the caller's stride (rounded up) when below the bound; an image that fits the rounded
     // row but not the caller's stride is refused below
-    const uint64_t dstride = ((jpeg_stride < bound ? jpeg_stride : bound) + 15) & ~(uint64_t)15;
-    const size_t len_bytes = ((size_t)n_reads * 4 + 255) & ~(size_t)255;
-    if ((st = ensure_device(ctx, &ctx->d_jpeg_out, &ctx->jpeg_out_bytes, len_bytes + (size_t)n_reads * dstride)) != MOCAP_OK) return st;
-    int32_t* d_len = reinterpret_cast<int32_t*>(ctx->d_jpeg_out);
-    uint8_t* d_jpeg = ctx->d_jpeg_out + len_bytes;
+    const uint64_t dstride = round_up(jpeg_stride < bound ? jpeg_stride : bound, 16);
+    int32_t* d_len;
+    uint8_t* d_jpeg;
+    st = grow_carved(ctx, ctx->jpeg_out, Drain::stream, [&](Layout& L) {
+        d_len = L.take<int32_t>(n_reads);
+        d_jpeg = L.take<uint8_t>((size_t)n_reads * dstride);
+    });
+    if (st) return st;
     // the live chain (live.cu), its frames kept on the device for the encoder
     LiveHostRun run;
     if ((st = live_host_run(ctx, tr, raw, n_reads, mode, timestamps, 1, (size_t)n_reads * 4, &run)) != MOCAP_OK) return st;
@@ -339,22 +318,18 @@ int mocap_live_jpeg_host(mocap_ctx* ctx, mocap_tracker* tr, const uint8_t* raw, 
                               r, (unsigned long long)jpeg_stride);
         total += (uint64_t)jpeg_len[r];
     }
-    if (total > ctx->jpeg_host_bytes) {
-        if (ctx->h_jpeg_out) cudaFreeHost(ctx->h_jpeg_out);
-        ctx->h_jpeg_out = nullptr; ctx->jpeg_host_bytes = 0;
-        CUDA_TRY(ctx, cudaHostAlloc(reinterpret_cast<void**>(&ctx->h_jpeg_out), total, cudaHostAllocDefault));
-        ctx->jpeg_host_bytes = total;
-    }
+    if ((st = ctx->jpeg_host.grow(ctx, total, Drain::none)) != MOCAP_OK) return st;     // the stream is idle here
+    uint8_t* h_jpeg = ctx->jpeg_host.as<uint8_t>();
     uint64_t at = 0;
     for (int r = 0; r < n_reads; ++r) {
-        CUDA_TRY(ctx, cudaMemcpyAsync(ctx->h_jpeg_out + at, d_jpeg + (size_t)r * dstride, (size_t)jpeg_len[r], cudaMemcpyDeviceToHost,
+        CUDA_TRY(ctx, cudaMemcpyAsync(h_jpeg + at, d_jpeg + (size_t)r * dstride, (size_t)jpeg_len[r], cudaMemcpyDeviceToHost,
                                       ctx->stream));
         at += (uint64_t)jpeg_len[r];
     }
     CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));                                        // synchronisation 2
     at = 0;
     for (int r = 0; r < n_reads; ++r) {
-        memcpy(jpeg + (size_t)r * jpeg_stride, ctx->h_jpeg_out + at, (size_t)jpeg_len[r]);
+        memcpy(jpeg + (size_t)r * jpeg_stride, h_jpeg + at, (size_t)jpeg_len[r]);
         at += (uint64_t)jpeg_len[r];
     }
     return MOCAP_OK;

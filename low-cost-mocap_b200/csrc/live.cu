@@ -82,7 +82,7 @@ int live_check(mocap_ctx* ctx, mocap_tracker* tr, const void* raw, int n_reads, 
     if ((mode & LIVE_LOCATE) && (!tr || !timestamps))
         return mocap_fail(ctx, MOCAP_EINVAL, "%s: LOCATE needs a tracker and timestamps", who);
     if (tr && tracker_context(tr) != ctx) return mocap_fail(ctx, MOCAP_EINVAL, "%s: the tracker belongs to another context", who);
-    if (!ctx->d_pp_m1) return mocap_fail(ctx, MOCAP_ESTATE, "mocap_set_preprocess has not been called");
+    if (!ctx->pp_in_w) return mocap_fail(ctx, MOCAP_ESTATE, "mocap_set_preprocess has not been called");
     if ((mode & LIVE_TRIANGULATE) && !ctx->cameras_set) return mocap_fail(ctx, MOCAP_ESTATE, "mocap_set_cameras has not been called");
     return MOCAP_OK;
 }
@@ -116,19 +116,6 @@ static int live_run(mocap_ctx* ctx, mocap_tracker* tr, const uint8_t* raw, int n
                                          reinterpret_cast<float*>(base + L.pos), reinterpret_cast<float*>(base + L.vel),
                                          reinterpret_cast<double*>(base + L.heading), base + L.present,
                                          reinterpret_cast<int32_t*>(base + L.chosen));
-}
-
-// grows a device buffer and its page-locked twin to at least `bytes` (after the stream drains)
-static int ensure_live_buffers(mocap_ctx* ctx, uint8_t** d, uint8_t** h, size_t* have, size_t bytes) {
-    if (bytes <= *have) return MOCAP_OK;
-    CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-    cudaFree(*d);
-    if (*h) cudaFreeHost(*h);
-    *d = nullptr; *h = nullptr; *have = 0;
-    CUDA_TRY(ctx, cudaMalloc(d, bytes));
-    CUDA_TRY(ctx, cudaHostAlloc(reinterpret_cast<void**>(h), bytes, cudaHostAllocDefault));
-    *have = bytes;
-    return MOCAP_OK;
 }
 
 extern "C" {
@@ -170,34 +157,42 @@ int live_host_run(mocap_ctx* ctx, mocap_tracker* tr, const uint8_t* raw, int n_r
     const int C = ctx->cfg.n_cam, S = ctx->cfg.width;
     mocap_live_offsets& L = run->L;
     live_offsets(ctx->cfg, n_reads, tr ? tracker_num_objects(tr) : 0, &L);
-    const size_t ts_bytes = (mode & LIVE_LOCATE) ? (((size_t)n_reads * sizeof(double) + 255) & ~(size_t)255) : 0;
     const size_t raw_bytes = (size_t)n_reads * C * ctx->pp_in_w * ctx->pp_in_h * 3;
-    run->res_bytes = (L.total + 255) & ~(size_t)255;
-    run->frame_bytes = keep_frames ? (((size_t)n_reads * C * S * S * 3 + 255) & ~(size_t)255) : 0;
     run->frame_copy = keep_frames ? (size_t)n_reads * C * S * S * 3 : 0;
     run->extra_bytes = extra_bytes;
-    if ((st = ensure_live_buffers(ctx, &ctx->d_live_in, &ctx->h_live_in, &ctx->live_in_bytes, ts_bytes + raw_bytes)) != MOCAP_OK) return st;
-    if ((st = ensure_live_buffers(ctx, &ctx->d_live_out, &ctx->h_live_out, &ctx->live_out_bytes,
-                                  run->res_bytes + run->frame_bytes + extra_bytes)) != MOCAP_OK) return st;
+    double* d_ts;
+    uint8_t *d_raw, *d_extra;
+    // device buffers and their page-locked twins, the same layout in both; the stream has drained if a device buffer grew
+    if ((st = grow_carved(ctx, ctx->live_in, Drain::stream, [&](Layout& R) {
+             d_ts = R.take<double>((mode & LIVE_LOCATE) ? n_reads : 0); d_raw = R.take<uint8_t>(raw_bytes); })) ||
+        (st = ctx->live_in_host.grow(ctx, ctx->live_in.bytes(), Drain::none)) ||
+        (st = grow_carved(ctx, ctx->live_out, Drain::stream, [&](Layout& R) {
+             R.take<uint8_t>(L.total);                             // the result, at offset 0
+             run->d_frames = R.take<uint8_t>(run->frame_copy); d_extra = R.take<uint8_t>(extra_bytes); })) ||
+        (st = ctx->live_out_host.grow(ctx, ctx->live_out.bytes(), Drain::none)))
+        return st;
+    run->frame_off = run->d_frames - ctx->live_out.as<uint8_t>();
+    run->extra_off = d_extra - ctx->live_out.as<uint8_t>();
+    if (!keep_frames) run->d_frames = nullptr;
     // the staging buffers are free here: the previous call returned after its synchronisation
-    if (ts_bytes) memcpy(ctx->h_live_in, timestamps, (size_t)n_reads * sizeof(double));
-    memcpy(ctx->h_live_in + ts_bytes, raw, raw_bytes);
-    CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_live_in, ctx->h_live_in, ts_bytes + raw_bytes, cudaMemcpyHostToDevice, ctx->stream));
-    run->d_frames = keep_frames ? ctx->d_live_out + run->res_bytes : nullptr;
-    return live_run(ctx, tr, ctx->d_live_in + ts_bytes, n_reads, mode, ts_bytes ? reinterpret_cast<const double*>(ctx->d_live_in) : nullptr,
-                    run->d_frames, ctx->d_live_out);
+    uint8_t* h_in = ctx->live_in_host.as<uint8_t>();
+    const size_t raw_off = d_raw - ctx->live_in.as<uint8_t>();
+    if (mode & LIVE_LOCATE) memcpy(h_in, timestamps, (size_t)n_reads * sizeof(double));
+    memcpy(h_in + raw_off, raw, raw_bytes);
+    CUDA_TRY(ctx, cudaMemcpyAsync(ctx->live_in.get(), h_in, raw_off + raw_bytes, cudaMemcpyHostToDevice, ctx->stream));
+    return live_run(ctx, tr, d_raw, n_reads, mode, (mode & LIVE_LOCATE) ? d_ts : nullptr, run->d_frames, ctx->live_out.get());
 }
 
 // the rest of mocap_live_host: the result, the frames (frames != NULL) and run.extra_bytes from the device pointer
 // `extra` back to the host, one synchronisation
 int live_host_finish(mocap_ctx* ctx, const LiveHostRun& run, uint8_t* frames, void* result, const void* extra, void* extra_out) {
-    uint8_t* h_extra = ctx->h_live_out + run.res_bytes + run.frame_bytes;
-    CUDA_TRY(ctx, cudaMemcpyAsync(ctx->h_live_out, ctx->d_live_out, run.L.total, cudaMemcpyDeviceToHost, ctx->stream));
-    if (frames) CUDA_TRY(ctx, cudaMemcpyAsync(ctx->h_live_out + run.res_bytes, run.d_frames, run.frame_copy, cudaMemcpyDeviceToHost, ctx->stream));
-    if (run.extra_bytes) CUDA_TRY(ctx, cudaMemcpyAsync(h_extra, extra, run.extra_bytes, cudaMemcpyDeviceToHost, ctx->stream));
+    uint8_t* h_out = ctx->live_out_host.as<uint8_t>();
+    CUDA_TRY(ctx, cudaMemcpyAsync(h_out, ctx->live_out.get(), run.L.total, cudaMemcpyDeviceToHost, ctx->stream));
+    if (frames) CUDA_TRY(ctx, cudaMemcpyAsync(h_out + run.frame_off, run.d_frames, run.frame_copy, cudaMemcpyDeviceToHost, ctx->stream));
+    if (run.extra_bytes) CUDA_TRY(ctx, cudaMemcpyAsync(h_out + run.extra_off, extra, run.extra_bytes, cudaMemcpyDeviceToHost, ctx->stream));
     CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-    memcpy(result, ctx->h_live_out, run.L.total);
-    if (frames) memcpy(frames, ctx->h_live_out + run.res_bytes, run.frame_copy);
-    if (run.extra_bytes) memcpy(extra_out, h_extra, run.extra_bytes);
+    memcpy(result, h_out, run.L.total);
+    if (frames) memcpy(frames, h_out + run.frame_off, run.frame_copy);
+    if (run.extra_bytes) memcpy(extra_out, h_out + run.extra_off, run.extra_bytes);
     return MOCAP_OK;
 }

@@ -122,17 +122,15 @@ static int ensure_match_split(mocap_ctx* ctx, int n_sets) {
     if (want * per_item > (512ll << 20)) want = (512ll << 20) / per_item;
     const int want_items = (int)want;
     if (n_sets <= ctx->match_cap_sets && want_items <= ctx->match_item_cap) return MOCAP_OK;
-    CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-    cudaFree(ctx->d_match_items); cudaFree(ctx->d_match_partial); cudaFree(ctx->d_match_range); cudaFree(ctx->d_match_arrive);
-    ctx->d_match_items = nullptr; ctx->d_match_partial = nullptr; ctx->d_match_range = nullptr; ctx->d_match_arrive = nullptr;
-    ctx->match_cap_sets = 0; ctx->match_item_cap = 0;
-    CUDA_TRY(ctx, cudaMalloc(&ctx->d_match_items, (size_t)want_items * sizeof(MatchItem)));
-    CUDA_TRY(ctx, cudaMalloc(&ctx->d_match_partial, (size_t)want_items * ctx->cfg.max_roots * MATCH_PARTIAL_WORDS * sizeof(unsigned long long)));
-    CUDA_TRY(ctx, cudaMalloc(&ctx->d_match_range, (size_t)want_items * 2 * sizeof(int)));
-    CUDA_TRY(ctx, cudaMalloc(&ctx->d_match_arrive, (size_t)n_sets * sizeof(unsigned)));
-    CUDA_TRY(ctx, cudaMemsetAsync(ctx->d_match_arrive, 0, (size_t)n_sets * sizeof(unsigned), ctx->stream));   // the finishers keep it zero
-    ctx->match_cap_sets = n_sets; ctx->match_item_cap = want_items;
-    return MOCAP_OK;
+    const size_t items = (size_t)want_items;
+    const int st = grow_carved(ctx, ctx->match_split, Drain::stream, [&](Layout& L) {
+        ctx->d_match_arrive = L.take<unsigned>(n_sets);      // the finishers keep it zero
+        L.zero_so_far();
+        ctx->d_match_items = L.take<MatchItem>(items); ctx->d_match_range = L.take<int>(items * 2);
+        ctx->d_match_partial = L.take<unsigned long long>(items * ctx->cfg.max_roots * MATCH_PARTIAL_WORDS);
+    });
+    ctx->match_cap_sets = st ? 0 : n_sets; ctx->match_item_cap = st ? 0 : want_items;
+    return st;
 }
 
 int launch_match(mocap_ctx* ctx, const int32_t* blob_xy, const int32_t* blob_n, int n_sets,
@@ -146,7 +144,7 @@ int launch_match(mocap_ctx* ctx, const int32_t* blob_xy, const int32_t* blob_n, 
     if (grid > full) grid = full;
     MatchSplit sp;
     memset(&sp, 0, sizeof(sp));
-    sp.counters = ctx->d_match_counter;
+    sp.counters = ctx->match_counter.as<unsigned>();
     if (ctx->match_chunk > 0) {
         const int st = ensure_match_split(ctx, n_sets);
         if (st) return st;
@@ -154,7 +152,7 @@ int launch_match(mocap_ctx* ctx, const int32_t* blob_xy, const int32_t* blob_n, 
         sp.partial = ctx->d_match_partial; sp.range = ctx->d_match_range; sp.arrive = ctx->d_match_arrive;
         sp.chunk = (uint32_t)ctx->match_chunk; sp.item_cap = (uint32_t)ctx->match_item_cap;
     }
-    CUDA_TRY(ctx, cudaMemsetAsync(ctx->d_match_counter, 0, 4 * sizeof(unsigned), ctx->stream));
+    CUDA_TRY(ctx, cudaMemsetAsync(ctx->match_counter.get(), 0, 4 * sizeof(unsigned), ctx->stream));
     k_match_triangulate<<<grid, warps * 32, smem, ctx->stream>>>(ctx->d_tables, blob_xy, blob_n, nullptr, nullptr, sp, n_sets, c.n_cam,
                                                                  c.max_blobs, c.max_roots, c.max_cands,
                                                                  (uint32_t)c.max_groups, obj, err, n_obj, set_flags, chosen, ctx->track_xy_cur, ctx->img_flags_cur);
@@ -206,7 +204,8 @@ int match_kernels_init(mocap_ctx* ctx) {
     CUDA_TRY(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_match_triangulate, 128, smem));
     ctx->match_ctas_per_sm = per_sm > 0 ? per_sm : 1;
     CUDA_TRY(ctx, cudaFuncSetAttribute(k_match_chunks, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    CUDA_TRY(ctx, cudaMalloc(&ctx->d_match_counter, 4 * sizeof(unsigned)));
+    int st = ctx->match_counter.grow(ctx, 4 * sizeof(unsigned), Drain::none);
+    if (st) return st;
     // candidate groups per item of the chunked matcher (match_device.cuh); MOCAP_MATCH_CHUNK=0: one warp per frame-set throughout
     const char* ch = getenv("MOCAP_MATCH_CHUNK");
     int chunk = ch && ch[0] ? atoi(ch) : MOCAP_MATCH_CHUNK;

@@ -115,21 +115,18 @@ __global__ void k_overlay_epiadvance(const uint32_t* __restrict__ counts, int n_
 int launch_epilines(mocap_ctx* ctx, uint8_t* frames, int n_sets, const int32_t* blob_xy, const int32_t* blob_n) {
     const mocap_config& g = ctx->cfg;
     if (n_sets <= 0 || g.n_cam < 2) return MOCAP_OK;
-    if (n_sets > ctx->line_counts_cap) {
-        CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-        cudaFree(ctx->d_line_counts);
-        ctx->d_line_counts = nullptr; ctx->line_counts_cap = 0;
-        CUDA_TRY(ctx, cudaMalloc(&ctx->d_line_counts, (size_t)n_sets * sizeof(uint32_t)));
-        ctx->line_counts_cap = n_sets;
-    }
+    const int st = ctx->line_counts.grow(ctx, (size_t)n_sets * sizeof(uint32_t), Drain::stream);
+    if (st) return st;
+    uint32_t* counts = ctx->line_counts.as<uint32_t>();
+    unsigned long long* counter = ctx->line_counter.as<unsigned long long>();
     const size_t smem = warp_state_bytes(g.max_roots, g.n_cam, g.max_cands, g.max_blobs);
     for (int pass = 0; pass < 2; ++pass) {
         k_overlay_epilines<<<dim3(n_sets, pass ? g.n_cam - 1 : 1), 32, smem, ctx->stream>>>(ctx->d_tables, blob_xy, blob_n, n_sets, g.n_cam, g.max_blobs, g.max_roots,
-                                                              g.max_cands, (uint32_t)g.max_groups, frames, g.width, g.height, ctx->d_palette,
-                                                              ctx->palette_len, ctx->d_line_counter, ctx->d_line_counts, pass);
+                                                              g.max_cands, (uint32_t)g.max_groups, frames, g.width, g.height, ctx->palette.as<uint8_t>(),
+                                                              ctx->palette_len, counter, counts, pass);
         CUDA_TRY(ctx, cudaGetLastError());
     }
-    k_overlay_epiadvance<<<1, 32, 0, ctx->stream>>>(ctx->d_line_counts, n_sets, ctx->d_line_counter);
+    k_overlay_epiadvance<<<1, 32, 0, ctx->stream>>>(counts, n_sets, counter);
     CUDA_TRY(ctx, cudaGetLastError());
     ctx->launches += 3;
     return MOCAP_OK;
@@ -158,13 +155,14 @@ int mocap_set_overlay(mocap_ctx* ctx, int on, uint32_t seed, int palette_len) {
     std::vector<uint8_t> pal((size_t)palette_len * 3);
     ov_palette(seed, palette_len, pal.data());
     CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-    if (!ctx->d_palette) CUDA_TRY(ctx, cudaMalloc(&ctx->d_palette, (size_t)MOCAP_OVERLAY_MAX_PALETTE * 3));
-    if (!ctx->d_line_counter) CUDA_TRY(ctx, cudaMalloc(&ctx->d_line_counter, sizeof(unsigned long long)));
+    int st = ctx->palette.grow(ctx, (size_t)MOCAP_OVERLAY_MAX_PALETTE * 3, Drain::none);
+    if (!st) st = ctx->line_counter.grow(ctx, sizeof(unsigned long long), Drain::none);
+    if (st) return st;
     const mocap_config& g = ctx->cfg;
     CUDA_TRY(ctx, cudaFuncSetAttribute(k_overlay_epilines, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                        (int)warp_state_bytes(g.max_roots, g.n_cam, g.max_cands, g.max_blobs)));
-    CUDA_TRY(ctx, cudaMemcpy(ctx->d_palette, pal.data(), pal.size(), cudaMemcpyHostToDevice));
-    CUDA_TRY(ctx, cudaMemset(ctx->d_line_counter, 0, sizeof(unsigned long long)));
+    CUDA_TRY(ctx, cudaMemcpy(ctx->palette.get(), pal.data(), pal.size(), cudaMemcpyHostToDevice));
+    CUDA_TRY(ctx, cudaMemset(ctx->line_counter.get(), 0, sizeof(unsigned long long)));
     ctx->palette_len = palette_len;
     ctx->overlay_on = on ? 1 : 0;
     return MOCAP_OK;
@@ -175,7 +173,7 @@ int mocap_overlay_dev(mocap_ctx* ctx, uint8_t* frames, int n_sets, const int32_t
     if (!frames || !blob_xy || !blob_n || n_sets < 0 || mode < 1 || (mode & ~(MOCAP_LIVE_CAPTURE | MOCAP_LIVE_TRIANGULATE)))
         return mocap_fail(ctx, MOCAP_EINVAL, "mocap_overlay_dev: bad argument (mode: CAPTURE and/or TRIANGULATE)");
     if ((mode & MOCAP_LIVE_TRIANGULATE) && !ctx->cameras_set) return mocap_fail(ctx, MOCAP_ESTATE, "mocap_set_cameras has not been called");
-    if ((mode & MOCAP_LIVE_TRIANGULATE) && !ctx->d_palette)
+    if ((mode & MOCAP_LIVE_TRIANGULATE) && !ctx->palette.get())
         return mocap_fail(ctx, MOCAP_ESTATE, "mocap_set_overlay has not been called (the epipolar lines need its palette)");
     if (n_sets == 0) return MOCAP_OK;
     CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));
@@ -191,9 +189,10 @@ int mocap_overlay_dev(mocap_ctx* ctx, uint8_t* frames, int n_sets, const int32_t
 static int overlay_frames(mocap_ctx* ctx, uint8_t* frames, int n_images, const int32_t* blob_xy, const int32_t* blob_n) {
     const size_t plane = (size_t)ctx->cfg.width * ctx->cfg.height;
     const int group = (int)((64ull << 20) / plane > 0 ? (64ull << 20) / plane : 1);     // images per grey scratch fill
-    int st = ensure_scratch(ctx, (size_t)(n_images < group ? n_images : group) * plane);
+    uint8_t* gray;
+    int st = grow_carved(ctx, ctx->scratch, Drain::stream,
+                         [&](Layout& L) { gray = L.take<uint8_t>((size_t)(n_images < group ? n_images : group) * plane); });
     if (st) return st;
-    uint8_t* gray = static_cast<uint8_t*>(ctx->d_scratch);
     for (int i0 = 0; i0 < n_images; i0 += group) {
         const int n = n_images - i0 < group ? n_images - i0 : group;
         uint8_t* f = frames + (size_t)i0 * plane * 3;

@@ -113,8 +113,8 @@ static int launch_preprocess(mocap_ctx* ctx, const uint8_t* raw_frames, int n_im
         uint8_t* g = gray ? gray + (size_t)i0 * S * S : nullptr;
         const int word_stores = (S % 4 == 0) && (reinterpret_cast<uintptr_t>(o) % 4 == 0) && (reinterpret_cast<uintptr_t>(g) % 4 == 0);
         k_preprocess<<<dim3((S + PP_TX - 1) / PP_TX, (S + PP_TY - 1) / PP_TY, groups * C), 256, 0, ctx->stream>>>(
-            raw_frames + (size_t)i0 * ctx->pp_in_w * ctx->pp_in_h * 3, n, C, ctx->pp_in_w, ctx->pp_in_h, S, ctx->d_pp_rot,
-            reinterpret_cast<const int32_t*>(ctx->d_pp_m1), ctx->d_pp_m2, o, g, word_stores);
+            raw_frames + (size_t)i0 * ctx->pp_in_w * ctx->pp_in_h * 3, n, C, ctx->pp_in_w, ctx->pp_in_h, S, ctx->pp_rot.as<int>(),
+            ctx->pp_m1.as<const int32_t>(), ctx->pp_m2.as<uint16_t>(), o, g, word_stores);
         CUDA_TRY(ctx, cudaGetLastError());
         ctx->launches += 1;
     }
@@ -133,10 +133,11 @@ int run_raw_groups(mocap_ctx* ctx, const uint8_t* raw_frames, int n_frame_sets, 
     const int C = ctx->cfg.n_cam, S = ctx->cfg.width;
     const size_t gray_bytes = (size_t)S * S;
     const int chunk = 4096 / C > 0 ? 4096 / C : 1;             // frame-sets per launch group (bounded scratch)
-    int st = ensure_scratch(ctx, (size_t)chunk * C * gray_bytes);
+    // the grey plane stays in the scratch through S1-S3, k_live_blobs and the overlay: none of them uses the scratch
+    uint8_t* gray;
+    int st = grow_carved(ctx, ctx->scratch, Drain::stream, [&](Layout& L) { gray = L.take<uint8_t>((size_t)chunk * C * gray_bytes); });
     if (st) return st;
     if (stages == RAW_DETECT && (st = ensure_images(ctx, (n_frame_sets < chunk ? n_frame_sets : chunk) * C)) != MOCAP_OK) return st;
-    uint8_t* gray = static_cast<uint8_t*>(ctx->d_scratch);
     for (int s0 = 0; s0 < n_frame_sets; s0 += chunk) {
         const int ns = n_frame_sets - s0 < chunk ? n_frame_sets - s0 : chunk;
         uint8_t* out = processed ? processed + (size_t)s0 * C * gray_bytes * 3 : nullptr;
@@ -178,14 +179,18 @@ int mocap_set_preprocess(mocap_ctx* ctx, int in_width, int in_height, const int*
     std::vector<uint16_t> m2((size_t)C * S * S);
     for (int c = 0; c < C; ++c) build_undistort_map(K + 9 * c, dist + 5 * c, S, m1.data() + (size_t)c * S * S * 2, m2.data() + (size_t)c * S * S);
     CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-    cudaFree(ctx->d_pp_m1); cudaFree(ctx->d_pp_m2); cudaFree(ctx->d_pp_rot);
-    ctx->d_pp_m1 = nullptr; ctx->d_pp_m2 = nullptr; ctx->d_pp_rot = nullptr;
-    CUDA_TRY(ctx, cudaMalloc(&ctx->d_pp_m1, m1.size() * sizeof(int16_t)));
-    CUDA_TRY(ctx, cudaMalloc(&ctx->d_pp_m2, m2.size() * sizeof(uint16_t)));
-    CUDA_TRY(ctx, cudaMalloc(&ctx->d_pp_rot, C * sizeof(int)));
-    CUDA_TRY(ctx, cudaMemcpy(ctx->d_pp_m1, m1.data(), m1.size() * sizeof(int16_t), cudaMemcpyHostToDevice));
-    CUDA_TRY(ctx, cudaMemcpy(ctx->d_pp_m2, m2.data(), m2.size() * sizeof(uint16_t), cudaMemcpyHostToDevice));
-    CUDA_TRY(ctx, cudaMemcpy(ctx->d_pp_rot, rotation, C * sizeof(int), cudaMemcpyHostToDevice));
+    // unset until all three maps are on the device, and unset with no maps if any step fails
+    ctx->pp_in_w = ctx->pp_in_h = 0;
+    ctx->pp_m1.reset(); ctx->pp_m2.reset(); ctx->pp_rot.reset();
+    const void* host[3] = {m1.data(), m2.data(), rotation};
+    const size_t bytes[3] = {m1.size() * sizeof(int16_t), m2.size() * sizeof(uint16_t), C * sizeof(int)};
+    DeviceBuffer* maps[3] = {&ctx->pp_m1, &ctx->pp_m2, &ctx->pp_rot};
+    for (int k = 0; k < 3; ++k) {
+        int st = maps[k]->grow(ctx, bytes[k], Drain::none);
+        if (!st && cudaMemcpy(maps[k]->get(), host[k], bytes[k], cudaMemcpyHostToDevice) != cudaSuccess)
+            st = mocap_fail(ctx, MOCAP_ECUDA, "mocap_set_preprocess: cudaMemcpy failed: %s", cudaGetErrorString(cudaGetLastError()));
+        if (st) { for (DeviceBuffer* m : maps) m->reset(); return st; }
+    }
     ctx->pp_in_w = in_width; ctx->pp_in_h = in_height;
     return MOCAP_OK;
 }
@@ -193,16 +198,16 @@ int mocap_set_preprocess(mocap_ctx* ctx, int in_width, int in_height, const int*
 int mocap_get_undistort_map(mocap_ctx* ctx, int cam, int16_t* m1, uint16_t* m2) {
     if (!ctx) return MOCAP_EINVAL;
     const int S = ctx->cfg.width;
-    if (!ctx->d_pp_m1 || cam < 0 || cam >= ctx->cfg.n_cam || !m1 || !m2) return mocap_fail(ctx, MOCAP_ESTATE, "mocap_get_undistort_map: no preprocessing set / bad argument");
-    CUDA_TRY(ctx, cudaMemcpy(m1, ctx->d_pp_m1 + (size_t)cam * S * S * 2, (size_t)S * S * 2 * sizeof(int16_t), cudaMemcpyDeviceToHost));
-    CUDA_TRY(ctx, cudaMemcpy(m2, ctx->d_pp_m2 + (size_t)cam * S * S, (size_t)S * S * sizeof(uint16_t), cudaMemcpyDeviceToHost));
+    if (!ctx->pp_in_w || cam < 0 || cam >= ctx->cfg.n_cam || !m1 || !m2) return mocap_fail(ctx, MOCAP_ESTATE, "mocap_get_undistort_map: no preprocessing set / bad argument");
+    CUDA_TRY(ctx, cudaMemcpy(m1, ctx->pp_m1.as<int16_t>() + (size_t)cam * S * S * 2, (size_t)S * S * 2 * sizeof(int16_t), cudaMemcpyDeviceToHost));
+    CUDA_TRY(ctx, cudaMemcpy(m2, ctx->pp_m2.as<uint16_t>() + (size_t)cam * S * S, (size_t)S * S * sizeof(uint16_t), cudaMemcpyDeviceToHost));
     return MOCAP_OK;
 }
 
 int mocap_preprocess_dev(mocap_ctx* ctx, const uint8_t* raw_frames, int n_images, uint8_t* out_frames) {
     if (!ctx) return MOCAP_EINVAL;
     if (!raw_frames || !out_frames || n_images < 0) return mocap_fail(ctx, MOCAP_EINVAL, "mocap_preprocess_dev: bad argument");
-    if (!ctx->d_pp_m1) return mocap_fail(ctx, MOCAP_ESTATE, "mocap_set_preprocess has not been called");
+    if (!ctx->pp_in_w) return mocap_fail(ctx, MOCAP_ESTATE, "mocap_set_preprocess has not been called");
     if (n_images == 0) return MOCAP_OK;
     CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));
     return launch_preprocess(ctx, raw_frames, n_images, out_frames, nullptr);
@@ -212,7 +217,7 @@ int mocap_pipeline_raw_dev(mocap_ctx* ctx, const uint8_t* raw_frames, int n_fram
                            double* obj, double* err, int32_t* n_obj, int32_t* set_flags) {
     if (!ctx) return MOCAP_EINVAL;
     if (!raw_frames || !obj || !err || !n_obj || n_frame_sets < 0) return mocap_fail(ctx, MOCAP_EINVAL, "mocap_pipeline_raw_dev: bad argument");
-    if (!ctx->d_pp_m1) return mocap_fail(ctx, MOCAP_ESTATE, "mocap_set_preprocess has not been called");
+    if (!ctx->pp_in_w) return mocap_fail(ctx, MOCAP_ESTATE, "mocap_set_preprocess has not been called");
     if (!ctx->cameras_set) return mocap_fail(ctx, MOCAP_ESTATE, "mocap_set_cameras has not been called");
     if (n_frame_sets == 0) return MOCAP_OK;
     CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));

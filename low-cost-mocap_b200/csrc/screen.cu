@@ -109,15 +109,15 @@ int mocap_screen_observations_host(mocap_ctx* ctx, const double* obs, const uint
     CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));
     const int C = ctx->cfg.n_cam;
     const int n = n_points ? (*n_points < 0 ? 0 : *n_points < n_points_max ? *n_points : n_points_max) : n_points_max;
-    auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
     const size_t rows = n > 0 ? (size_t)n : 1;
-    const size_t b_obs = al(rows * C * 2 * 8), b_mask = al(rows * C), b_R = al((size_t)C * 9 * 8), b_t = al((size_t)C * 3 * 8);
-    st = ensure_scratch(ctx, b_obs + 2 * b_mask + b_R + b_t + al(4 * sizeof(int32_t)));
+    double *d_obs, *d_R, *d_t;
+    uint8_t *d_in, *d_out;
+    int32_t* d_stats;
+    st = grow_carved(ctx, ctx->scratch, Drain::stream, [&](Layout& L) {
+        d_obs = L.take<double>(rows * C * 2); d_in = L.take<uint8_t>(rows * C); d_out = L.take<uint8_t>(rows * C);
+        d_R = L.take<double>((size_t)C * 9); d_t = L.take<double>((size_t)C * 3); d_stats = L.take<int32_t>(4);
+    });
     if (st) return st;
-    unsigned char* p = static_cast<unsigned char*>(ctx->d_scratch);
-    double* d_obs = (double*)p; p += b_obs; uint8_t* d_in = p; p += b_mask; uint8_t* d_out = p; p += b_mask;
-    double* d_R = (double*)p; p += b_R; double* d_t = (double*)p; p += b_t;
-    int32_t* d_stats = (int32_t*)p;
     cudaStream_t s = ctx->stream;
     if (n > 0) {
         CUDA_TRY(ctx, cudaMemcpyAsync(d_obs, obs, (size_t)n * C * 2 * 8, cudaMemcpyHostToDevice, s));
