@@ -10,71 +10,24 @@ device takes differently because of rounding (nvcc contracts to fused multiply-a
 -ffp-contract=off) from a wrong one."""
 import ctypes
 import importlib
-import os
-import subprocess
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-HC = os.path.join(ROOT, "tests", "hostcheck")
+from tests import hostbuild
+from tests.hostbuild import ptr
+
 synth = importlib.import_module("low-cost-mocap_b200.synth")
-P = ctypes.c_void_p
-_I = ctypes.c_int
-_D = ctypes.c_double
 SCALE_PX = 4.0          # CG_SCALE_PX: the Cauchy scale of the graph's translation weights
-
-
-def p(a):
-    return a.ctypes.data_as(P)
 
 
 def c64(a):
     return np.ascontiguousarray(a, dtype=np.float64)
 
 
-def _gxx(src, out):
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-shared", "-fPIC", "-ffp-contract=off", "-o", out, os.path.join(HC, src), "-lm"])
-    return ctypes.CDLL(out)
-
-
-def build_ransac_host(tmpdir):
-    """g++ build of csrc/calib_ransac.cuh (tests/hostcheck/calib_ransac_host.cpp) -> ctypes library."""
-    lib = _gxx("calib_ransac_host.cpp", os.path.join(str(tmpdir), "libcalib_ransac_host.so"))
-    lib.hc_seven_point.argtypes = [P, P, P]
-    lib.hc_fm_error.argtypes = [P, P, _I, P]
-    lib.hc_inlier_mask.argtypes = [P, P, _I, _D, P]
-    lib.hc_draw7.argtypes = [ctypes.c_uint64, _I, _I, _I, _I, _I, P]
-    lib.hc_has_collinear.argtypes = [P]
-    lib.hc_ransac_select.argtypes = [P, _I, _I, _I, ctypes.c_uint64, _D, P, P, P]
-    lib.hc_ransac_models.argtypes = [P, _I, _I, _I, ctypes.c_uint64, _D, P, P, P]
-    lib.hc_ransac_models.restype = None
-    return lib
-
-
-def build_graph_host(tmpdir):
-    """g++ build of csrc/calib_graph.cuh and calib_pose.h (tests/hostcheck/calib_graph_host.cpp) -> ctypes library."""
-    lib = _gxx("calib_graph_host.cpp", os.path.join(str(tmpdir), "libcalib_graph_host.so"))
-    lib.hc_track_block.argtypes = [P, P, P, P, _I, P]
-    lib.hc_track_block.restype = _I
-    lib.hc_cheirality.argtypes = [P, P, P, P] + [_D] * 4 + [P]
-    lib.hc_cheirality.restype = _D
-    lib.hc_cheirality_pair.argtypes = [P, P, P, P, P, P, _I, P, P, P]
-    lib.hc_cheirality_pair.restype = None
-    lib.hc_fit_from_normal.argtypes = [P, P, P]
-    lib.hc_fit_from_normal.restype = _I
-    lib.hc_motion_from_essential.argtypes = [P, P, P]
-    lib.hc_motion_from_essential.restype = None
-    lib.hc_rotation_average.argtypes = [_I, _I, P, P, P, P, _D, P, P, P]
-    lib.hc_rotation_average.restype = _I
-    lib.hc_translations.argtypes = [P, P, _I, _I, P, P, P, _I, _D, P, P]
-    lib.hc_translations.restype = _I
-    return lib
-
-
 class Libs:
-    def __init__(self, tmpdir):
-        self.rs = build_ransac_host(tmpdir)
-        self.cg = build_graph_host(tmpdir)
+    """The host builds the model calls: rs of csrc/calib_ransac.cuh, cg of csrc/calib_graph.cuh and calib_pose.h."""
+    def __init__(self):
+        self.rs, self.cg = hostbuild.load("calib_ransac"), hostbuild.load("calib_graph")
 
 
 # ------------------------------------------------------------------------------------------------------------ inputs
@@ -132,7 +85,7 @@ def host_ransac(libs, pts, pair, H, seed, thr):
     F = np.zeros(9)
     mask = np.zeros(m, dtype=np.uint8)
     cnt = ctypes.c_int(0)
-    ok = libs.rs.hc_ransac_select(p(pts), m, pair, H, seed, thr, p(F), p(mask), ctypes.byref(cnt)) == 1
+    ok = libs.rs.hc_ransac_select(ptr(pts), m, pair, H, seed, thr, ptr(F), ptr(mask), ctypes.byref(cnt)) == 1
     return {"ok": ok, "F": F.reshape(3, 3), "mask": mask.astype(bool), "count": cnt.value if ok else 0,
             "margin": ransac_margin(F, pts, thr) if ok else np.full(m, np.inf)}
 
@@ -142,7 +95,7 @@ def ransac_models(libs, pts, pair, H, seed, thr):
     n = np.zeros(H, dtype=np.int32)
     counts = np.zeros((H, 3), dtype=np.int32)
     F = np.zeros((H, 3, 3, 3))
-    libs.rs.hc_ransac_models(p(pts), len(pts), pair, H, seed, thr, p(n), p(counts), p(F))
+    libs.rs.hc_ransac_models(ptr(pts), len(pts), pair, H, seed, thr, ptr(n), ptr(counts), ptr(F))
     return n, counts, F
 
 
@@ -184,7 +137,7 @@ def fit_product(libs):
     """The product's host fit (hc_fit_from_normal: trf::sym_eig and svd3, the product's sign) on the numpy normal matrix."""
     def fit(x1, x2, inl, T):
         F = np.zeros(9)
-        assert libs.cg.hc_fit_from_normal(p(normal45(x1, x2, inl, T)), p(c64(T)), p(F)) == 1
+        assert libs.cg.hc_fit_from_normal(ptr(normal45(x1, x2, inl, T)), ptr(c64(T)), ptr(F)) == 1
         return F.reshape(3, 3)
     return fit
 
@@ -242,7 +195,7 @@ def dlt(Pa, Pb, xa, xb):
 
 def motions(libs, E):
     Rs, ts = np.zeros((4, 9)), np.zeros((4, 3))
-    libs.cg.hc_motion_from_essential(p(c64(E)), p(Rs), p(ts))
+    libs.cg.hc_motion_from_essential(ptr(c64(E)), ptr(Rs), ptr(ts))
     return Rs.reshape(4, 3, 3), ts
 
 
@@ -353,8 +306,8 @@ def graph_model(libs, obs, mask, Ks, H=2048, seed=0, thr=1.0, **options):
         for q in range(4):
             front = np.zeros(len(pts), dtype=np.uint8)
             ang, marg = np.zeros(len(pts)), np.zeros(len(pts))
-            libs.cg.hc_cheirality_pair(p(c64(Ks[a])), p(c64(Ks[b])), p(c64(Rs[q])), p(c64(ts[q])), p(pts), p(inl8), len(pts),
-                                       p(front), p(ang), p(marg))
+            libs.cg.hc_cheirality_pair(ptr(c64(Ks[a])), ptr(c64(Ks[b])), ptr(c64(Rs[q])), ptr(c64(ts[q])), ptr(pts), ptr(inl8), len(pts),
+                                       ptr(front), ptr(ang), ptr(marg))
             counts[q] = front.sum()
             angs.append(ang)
             mg["front"] = min(mg["front"], marg.min())
@@ -378,8 +331,8 @@ def graph_model(libs, obs, mask, Ks, H=2048, seed=0, thr=1.0, **options):
     ib = np.array([x[1] for x in table], dtype=np.int32)
     R = np.zeros((C, 3, 3))
     resid = np.zeros(len(table))
-    assert libs.cg.hc_rotation_average(C, len(table), p(ia), p(ib), p(c64(Rab)), p(c64(wrot)), o["rot_outlier_deg"], p(use), p(R),
-                                       p(resid)) == 1
+    assert libs.cg.hc_rotation_average(C, len(table), ptr(ia), ptr(ib), ptr(c64(Rab)), ptr(c64(wrot)), o["rot_outlier_deg"], ptr(use), ptr(R),
+                                       ptr(resid)) == 1
     for p_, rep in enumerate(pairs):
         rep["used"] = int(use[p_])
         if rep["candidate"] >= 0:
@@ -399,7 +352,7 @@ def graph_model(libs, obs, mask, Ks, H=2048, seed=0, thr=1.0, **options):
     f = c64([k[0, 0] for k in Ks])
     t = np.zeros((C, 3))
     w = np.zeros((n, C))
-    assert libs.cg.hc_translations(p(c64(obs)), p(init), n, C, p(Kinv), p(c64(R)), p(f), o["irls_rounds"], SCALE_PX, p(t), p(w)) == 1
+    assert libs.cg.hc_translations(ptr(c64(obs)), ptr(init), n, C, ptr(Kinv), ptr(c64(R)), ptr(f), o["irls_rounds"], SCALE_PX, ptr(t), ptr(w)) == 1
     keep = (w >= 0.5).sum(1) >= 2
     support = ((w >= 0.5) & keep[:, None]).astype(np.uint8)
     wm = np.abs(w[init.astype(bool)] - 0.5) / 0.5

@@ -7,10 +7,10 @@ import numpy as np
 
 root, lib_path, case = sys.argv[1], sys.argv[2], sys.argv[3]
 sys.path.insert(0, root)
+from tests.hostbuild import bind, ptr  # noqa: E402
 from tests.util import load_golden  # noqa: E402
 
-lib = ctypes.CDLL(lib_path)
-p = lambda a: a.ctypes.data_as(ctypes.c_void_p)
+lib = bind(ctypes.CDLL(lib_path), "fused_emu")
 z = load_golden(case, n=4)
 C, B = int(z["C"]), 4
 frames = np.ascontiguousarray(z["frames"][:B])
@@ -23,6 +23,6 @@ RM, MB, E = 128, 64, 1024
 obj = np.zeros((B, RM, 3)); err = np.zeros((B, RM)); k = np.zeros(B, np.int32); fl = np.zeros(B, np.int32)
 bxy = np.zeros((B * C, MB, 2), np.int32); bn = np.zeros(B * C, np.int32)
 iw = np.zeros(B * C, np.uint32); sw = np.zeros(B, np.uint32); cnt = np.zeros(4, np.int64)
-rc = lib.hc_pipeline_fused(p(frames), B, C, 640, 480, 51, p(K), p(R), p(t), MB, E, RM, 8, ctypes.c_uint(4096), 8, 2,
-                           p(obj), p(err), p(k), p(fl), p(bxy), p(bn), p(iw), p(sw), p(cnt), 1)
+rc = lib.hc_pipeline_fused(ptr(frames), B, C, 640, 480, 51, ptr(K), ptr(R), ptr(t), MB, E, RM, 8, ctypes.c_uint(4096), 8, 2,
+                           ptr(obj), ptr(err), ptr(k), ptr(fl), ptr(bxy), ptr(bn), ptr(iw), ptr(sw), ptr(cnt), 1)
 print("RESULT", rc, cnt.tolist(), k.tolist())

@@ -2,17 +2,16 @@
 csrc/locate_kernels.cu) and the golden generator tests/golden/make_golden_locate.py: seeded scenes that reach every
 branch of the greedy scan (crowded rigs, shared markers, tolerance edges ulp by ulp, heading folds, the drone-index
 edge, count limits, non-finite rows, random fuzz), the oracle on a scene as arrays, a trace of which points the scan
-picked (for the reach statistics), the g++ build of the device code and the comparison both test tiers use.
+picked (for the reach statistics) and the comparison both test tiers use.
 
 A scene is (points f64 [K, 3], errors f64 [K]); a batch is (obj f64 [B, R, 3], err f64 [B, R], n int32 [B]) in the
 layout mocap_locate_objects_dev reads, its rows beyond n filled with a marker triplet that must be ignored."""
-import ctypes
 import os
-import subprocess
 
 import numpy as np
 
 from oracle.ref_port import RefPort
+from tests.hostbuild import ptr
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden", "locate_edge.npz")
@@ -348,18 +347,6 @@ def trace(pts):
     return out
 
 
-# ---------------------------------------------------------------------------------------------- host build
-def build_locate_host(tmpdir):
-    """g++ build of csrc/locate_device.cuh (tests/hostcheck/locate_host.cpp) -> ctypes library."""
-    out = os.path.join(str(tmpdir), "liblocate_host.so")
-    subprocess.check_call(["g++", "-O2", "-shared", "-fPIC", "-ffp-contract=off", "-std=c++17", "-o", out,
-                           os.path.join(ROOT, "tests", "hostcheck", "locate_host.cpp"), "-lm"])
-    lib = ctypes.CDLL(out)
-    P, I = ctypes.c_void_p, ctypes.c_int
-    lib.hc_locate.restype, lib.hc_locate.argtypes = None, [P, P, P, I, I, I, P, P, P]
-    return lib
-
-
 SENTINEL_F, SENTINEL_I = -7.25e300, -123456789
 GUARD = 3                                          # sentinel rows after every frame-set's records
 
@@ -383,10 +370,9 @@ def host_locate(lib, obj, err, n, max_roots, max_objects):
     obj = np.ascontiguousarray(obj, np.float64); err = np.ascontiguousarray(err, np.float64); n = np.ascontiguousarray(n, np.int32)
     B = len(n)
     rec, di, cnt = guarded_outputs(B, max_objects)
-    p = lambda a: a.ctypes.data_as(ctypes.c_void_p)
     # frame-set s writes rec[s, :max_objects]: the library sees a batch of one whose outputs start at that row
     for s in range(B):
-        lib.hc_locate(p(obj[s:]), p(err[s:]), p(n[s:]), 1, max_roots, max_objects, p(rec[s:]), p(di[s:]), p(cnt[s:]))
+        lib.hc_locate(ptr(obj[s:]), ptr(err[s:]), ptr(n[s:]), 1, max_roots, max_objects, ptr(rec[s:]), ptr(di[s:]), ptr(cnt[s:]))
     check_guards(rec, di, cnt, B, max_objects)
     return {"objects": rec[:B, :max_objects].copy(), "drone_index": di[:B, :max_objects].copy(), "n": cnt[:B].copy()}
 
@@ -398,8 +384,7 @@ def host_locate_batch(lib, obj, err, n, max_roots, max_objects):
     B = len(n)
     rec = np.full((B + 1, max_objects, 5), SENTINEL_F); di = np.full((B + 1, max_objects), SENTINEL_I, np.int32)
     cnt = np.full(B + 1, SENTINEL_I, np.int32)
-    p = lambda a: a.ctypes.data_as(ctypes.c_void_p)
-    lib.hc_locate(p(obj), p(err), p(n), B, max_roots, max_objects, p(rec), p(di), p(cnt))
+    lib.hc_locate(ptr(obj), ptr(err), ptr(n), B, max_roots, max_objects, ptr(rec), ptr(di), ptr(cnt))
     assert (rec[B] == SENTINEL_F).all() and (di[B] == SENTINEL_I).all() and cnt[B] == SENTINEL_I
     return {"objects": rec[:B], "drone_index": di[:B], "n": cnt[:B]}
 

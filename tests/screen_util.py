@@ -1,13 +1,11 @@
 """Helpers shared by the CPU and GPU tests of the per-view screen (csrc/screen.cuh) and tools/screen_threshold_probe.py:
-contaminated calibration tracks, the g++ build of the screen and the inputs both test tiers use."""
-import ctypes
+contaminated calibration tracks, the host build's screen and the inputs both test tiers use."""
 import importlib
-import os
-import subprocess
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from tests.hostbuild import ptr
+
 synth = importlib.import_module("low-cost-mocap_b200.synth")
 
 
@@ -32,20 +30,6 @@ def contaminated_tracks(C, n, frac, seed):
     return obs, mask, out, bad, poses, K, pts
 
 
-def build_screen_host(tmpdir):
-    """g++ build of csrc/screen.cuh (tests/hostcheck/screen_host.cpp) -> ctypes library."""
-    out = os.path.join(str(tmpdir), "libscreen_host.so")
-    subprocess.check_call(["g++", "-O2", "-shared", "-fPIC", "-ffp-contract=off", "-o", out,
-                           os.path.join(ROOT, "tests", "hostcheck", "screen_host.cpp"), "-lm"])
-    lib = ctypes.CDLL(out)
-    P = ctypes.c_void_p
-    lib.hc_screen.argtypes = [P, P, ctypes.c_int, ctypes.c_int, P, P, P, ctypes.c_double, P, P]
-    lib.hc_screen.restype = None
-    lib.hc_screen_pair.argtypes = [ctypes.c_uint, ctypes.c_int]
-    lib.hc_screen_pair.restype = ctypes.c_uint
-    return lib
-
-
 def poses_arrays(poses):
     R = np.ascontiguousarray(np.stack([np.asarray(p["R"], dtype=np.float64).reshape(3, 3) for p in poses]))
     t = np.ascontiguousarray(np.stack([np.asarray(p["t"], dtype=np.float64).reshape(3) for p in poses]))
@@ -61,8 +45,7 @@ def host_screen(lib, obs, mask, Ks, poses, thr):
     R, t = poses_arrays(poses)
     out = np.zeros_like(mask)
     stats = np.zeros(4, dtype=np.int32)
-    p = lambda a: a.ctypes.data_as(ctypes.c_void_p)
-    lib.hc_screen(p(obs), p(mask), n, C, p(K), p(R), p(t), float(thr), p(out), p(stats))
+    lib.hc_screen(ptr(obs), ptr(mask), n, C, ptr(K), ptr(R), ptr(t), float(thr), ptr(out), ptr(stats))
     return out, stats
 
 

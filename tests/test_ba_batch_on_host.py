@@ -3,38 +3,22 @@ the SIMT emulation: several problems on sub-grids of one launch, each with its o
 problem must give the same bits (poses and report) as the single-solve hook on a grid of its own CTA count."""
 import ctypes
 import os
-import subprocess
 
 import numpy as np
 import pytest
 from scipy.spatial.transform import Rotation
 
+from tests import hostbuild
+from tests.hostbuild import ptr
 from tests.util import ROOT
 
-HC = os.path.join(ROOT, "tests", "hostcheck")
-CUDA_INC = os.path.join(os.environ.get("CUDA_HOME", "/usr/local/cuda"), "include")
-_P = ctypes.c_void_p
 KEYS = ["cost_initial", "cost_final", "optimality", "n_iterations", "n_fev", "status", "n_residuals", "prefit_cost_initial",
         "prefit_cost_final", "prefit_iterations", "smem", "n_tr_solves", "n_tr_newton"]
 
 
 @pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    d = tmp_path_factory.mktemp("ba_batch_emu")
-    libs = {}
-    for name, src in (("single", "ba_dev_emu_host.cpp"), ("batch", "ba_batch_emu_host.cpp")):
-        out = str(d / f"lib{name}.so")
-        subprocess.check_call(["g++", "-std=c++20", "-O2", "-shared", "-fPIC", "-pthread", "-I" + CUDA_INC, "-Wno-attributes",
-                               "-Wno-unknown-pragmas", "-fno-strict-aliasing", "-o", out, os.path.join(HC, src)])
-        libs[name] = ctypes.CDLL(out)
-    libs["single"].hc_ba_solve_dev.argtypes = [_P] * 2 + [ctypes.c_int] * 2 + [_P] * 3 + [ctypes.c_double] + [ctypes.c_int] * 6 + [_P]
-    libs["batch"].hc_ba_solve_batch.argtypes = [ctypes.c_int, _P, _P, _P, ctypes.c_int, _P, _P, _P, ctypes.c_double] + \
-        [ctypes.c_int] * 4 + [_P, ctypes.c_int, _P]
-    return libs
-
-
-def _p(a):
-    return a.ctypes.data_as(_P)
+def emu():
+    return {"single": hostbuild.load("ba_dev_emu"), "batch": hostbuild.load("ba_batch_emu")}
 
 
 def _single(emu, prob, K, prefit, n_ctas, n_threads, jac_mode=1):
@@ -43,8 +27,8 @@ def _single(emu, prob, K, prefit, n_ctas, n_threads, jac_mode=1):
     Ks = np.ascontiguousarray(np.stack([K] * C))
     R, t = R.copy(), t.copy()
     rep = np.zeros(13)
-    assert emu["single"].hc_ba_solve_dev(_p(obs), _p(mask), obs.shape[0], C, _p(Ks), _p(R), _p(t), 1e-2, 0, jac_mode, int(prefit), 50,
-                                         n_ctas, n_threads, _p(rep)) == 0
+    assert emu["single"].hc_ba_solve_dev(ptr(obs), ptr(mask), obs.shape[0], C, ptr(Ks), ptr(R), ptr(t), 1e-2, 0, jac_mode, int(prefit), 50,
+                                         n_ctas, n_threads, ptr(rep)) == 0
     return R, t, rep
 
 
@@ -59,8 +43,8 @@ def _batch(emu, probs, K, prefit, ctas, n_threads, jac_mode=1):
     arr = lambda xs: (ctypes.c_void_p * n)(*[x.ctypes.data for x in xs])
     m = np.array([p[0].shape[0] for p in probs], dtype=np.int32)
     c = np.array(ctas, dtype=np.int32)
-    assert emu["batch"].hc_ba_solve_batch(n, arr(keep[0::2]), arr(keep[1::2]), _p(m), C, _p(Ks), arr(Rs), arr(ts), 1e-2, 0, jac_mode,
-                                          int(prefit), 50, _p(c), n_threads, arr(reps)) == 0
+    assert emu["batch"].hc_ba_solve_batch(n, arr(keep[0::2]), arr(keep[1::2]), ptr(m), C, ptr(Ks), arr(Rs), arr(ts), 1e-2, 0, jac_mode,
+                                          int(prefit), 50, ptr(c), n_threads, arr(reps)) == 0
     return list(zip(Rs, ts, reps))
 
 

@@ -7,44 +7,22 @@ machine without a GPU.
   tests/hostcheck/simt_emu.h) against the model, iteration by iteration: `prefit_max_iter = k` with `max_nfev = 1`
   returns the poses after k prefit iterations (the polish evaluates once and takes no step).
 * A camera that sees no point: it is held where it is, and the others are fitted as if it were not in the rig."""
-import ctypes
-import os
-import subprocess
-
 import numpy as np
 import pytest
 from scipy.spatial.transform import Rotation
 
 from tests import ba_prefit_util as bu
+from tests import hostbuild
+from tests.hostbuild import ptr
 from tests.util import ROOT, synth
 
-HC = os.path.join(ROOT, "tests", "hostcheck")
-CUDA_INC = os.path.join(os.environ.get("CUDA_HOME", "/usr/local/cuda"), "include")
-_P = ctypes.c_void_p
 KEYS = ["cost_initial", "cost_final", "optimality", "n_iterations", "n_fev", "status", "n_residuals", "prefit_cost_initial",
         "prefit_cost_final", "prefit_iterations", "smem", "n_tr_solves", "n_tr_newton"]
 
 
-def _p(a):
-    return a.ctypes.data_as(_P)
-
-
-def _gxx(out, src):
-    subprocess.check_call(["g++", "-std=c++20", "-O2", "-shared", "-fPIC", "-pthread", "-I" + CUDA_INC, "-Wno-attributes",
-                           "-Wno-unknown-pragmas", "-fno-strict-aliasing", "-o", out, os.path.join(HC, src)])
-    return ctypes.CDLL(out)
-
-
 @pytest.fixture(scope="module")
-def libs(tmp_path_factory):
-    d = tmp_path_factory.mktemp("ba_prefit")
-    emu = _gxx(str(d / "libba_dev_emu.so"), "ba_dev_emu_host.cpp")
-    emu.hc_ba_solve_dev.argtypes = [_P] * 2 + [ctypes.c_int] * 2 + [_P] * 3 + [ctypes.c_double] + [ctypes.c_int] * 6 + [_P]
-    parts = _gxx(str(d / "libba_parts.so"), "ba_parts_host.cpp")
-    for f in ("hc_ba_exp_so3", "hc_ba_rotvec_to_matrix", "hc_ba_matrix_to_rotvec", "hc_trf_rotvec_to_matrix", "hc_trf_matrix_to_rotvec"):
-        getattr(parts, f).argtypes = [_P] * 2
-    parts.hc_ba_view_jacobian.argtypes = [_P] * 5
-    return emu, parts
+def libs():
+    return hostbuild.load("ba_dev_emu"), hostbuild.load("ba_parts")
 
 
 def solve(emu, obs, mask, K, R, t, prefit_max_iter=50, max_nfev=1, n_ctas=2, n_threads=64, prefit=True):
@@ -55,8 +33,8 @@ def solve(emu, obs, mask, K, R, t, prefit_max_iter=50, max_nfev=1, n_ctas=2, n_t
     Ks = np.ascontiguousarray(np.stack([K] * C) if K.ndim == 2 else K)
     R = np.ascontiguousarray(np.array(R, np.float64)); t = np.ascontiguousarray(np.array(t, np.float64).reshape(C, 3))
     rep = np.zeros(13)
-    assert emu.hc_ba_solve_dev(_p(obs), _p(mask), obs.shape[0], C, _p(Ks), _p(R), _p(t), 1e-2, max_nfev, 1, int(prefit),
-                               prefit_max_iter, n_ctas, n_threads, _p(rep)) == 0
+    assert emu.hc_ba_solve_dev(ptr(obs), ptr(mask), obs.shape[0], C, ptr(Ks), ptr(R), ptr(t), 1e-2, max_nfev, 1, int(prefit),
+                               prefit_max_iter, n_ctas, n_threads, ptr(rep)) == 0
     return R, t, dict(zip(KEYS, rep))
 
 
@@ -115,7 +93,7 @@ def test_view_jacobian_equals_complex_step(libs, where):
     uv = np.array([u + 3.0, v - 2.0])
     Rt = np.ascontiguousarray(np.c_[R, t])
     out = np.zeros(20)
-    parts.hc_ba_view_jacobian(_p(Rt), _p(K4), _p(np.ascontiguousarray(X)), _p(uv), _p(out))
+    parts.hc_ba_view_jacobian(ptr(Rt), ptr(K4), ptr(np.ascontiguousarray(X)), ptr(uv), ptr(out))
     e_ref, J_ref = _cs_view(Rt, K4, X, uv)
     scale = np.abs(J_ref).max()
     assert np.abs(out[:2] - e_ref).max() < 1e-9
@@ -135,7 +113,7 @@ def test_exp_so3_equals_scipy(libs, angle):
         a = rng.normal(size=3)
         w = np.ascontiguousarray(a / np.linalg.norm(a) * angle)
         E = np.zeros(9)
-        parts.hc_ba_exp_so3(_p(w), _p(E))
+        parts.hc_ba_exp_so3(ptr(w), ptr(E))
         assert np.abs(E.reshape(3, 3) - Rotation.from_rotvec(w).as_matrix()).max() < 1e-15
 
 
@@ -161,15 +139,15 @@ def test_rotvec_conversions_equal_scipy_and_trf(libs):
     branches = set()
     for rv in _rotvecs():
         R, R2 = np.zeros(9), np.zeros(9)
-        parts.hc_ba_rotvec_to_matrix(_p(rv), _p(R))
-        parts.hc_trf_rotvec_to_matrix(_p(rv), _p(R2))
+        parts.hc_ba_rotvec_to_matrix(ptr(rv), ptr(R))
+        parts.hc_trf_rotvec_to_matrix(ptr(rv), ptr(R2))
         ref = Rotation.from_rotvec(rv).as_matrix()
         assert np.array_equal(R, R2) and np.abs(R.reshape(3, 3) - ref).max() < 1e-15
         Rm = np.ascontiguousarray(ref.reshape(9))
         branches.add(int(np.argmax([Rm[0], Rm[4], Rm[8], Rm[0] + Rm[4] + Rm[8]])))
         v, v2 = np.zeros(3), np.zeros(3)
-        parts.hc_ba_matrix_to_rotvec(_p(Rm), _p(v))
-        parts.hc_trf_matrix_to_rotvec(_p(Rm), _p(v2))
+        parts.hc_ba_matrix_to_rotvec(ptr(Rm), ptr(v))
+        parts.hc_trf_matrix_to_rotvec(ptr(Rm), ptr(v2))
         vref = Rotation.from_matrix(ref).as_rotvec()
         assert np.array_equal(v, v2)
         if np.linalg.norm(vref) > np.pi - 1e-6:          # at pi, w and -w are the same turn

@@ -4,41 +4,21 @@ recover the true rig from noise-free tracks, and on a 16-camera rig where the re
 pair-frame cheirality picks the true motion of every pair."""
 import ctypes
 import importlib
-import os
-import subprocess
 
 import cv2
 import numpy as np
 import pytest
 
 from oracle.ref_port import RefPort
+from tests import hostbuild
+from tests.hostbuild import ptr
 
 synth = importlib.import_module("low-cost-mocap_b200.synth")
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-P = ctypes.c_void_p
 
 
 @pytest.fixture(scope="module")
-def lib(tmp_path_factory):
-    out = os.path.join(str(tmp_path_factory.mktemp("calib_graph")), "libcalib_graph_host.so")
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-shared", "-fPIC", "-ffp-contract=off", "-o", out,
-                           os.path.join(ROOT, "tests", "hostcheck", "calib_graph_host.cpp"), "-lm"])
-    lib = ctypes.CDLL(out)
-    lib.hc_track_block.argtypes = [P, P, P, P, ctypes.c_int, P]
-    lib.hc_track_block.restype = ctypes.c_int
-    lib.hc_cheirality.argtypes = [P, P, P, P] + [ctypes.c_double] * 4 + [P]
-    lib.hc_cheirality.restype = ctypes.c_double
-    lib.hc_motion_from_essential.argtypes = [P, P, P]
-    lib.hc_motion_from_essential.restype = None
-    lib.hc_rotation_average.argtypes = [ctypes.c_int, ctypes.c_int, P, P, P, P, ctypes.c_double, P, P, P]
-    lib.hc_rotation_average.restype = ctypes.c_int
-    lib.hc_translations.argtypes = [P, P, ctypes.c_int, ctypes.c_int, P, P, P, ctypes.c_int, ctypes.c_double, P, P]
-    lib.hc_translations.restype = ctypes.c_int
-    return lib
-
-
-def p(a):
-    return a.ctypes.data_as(P)
+def lib():
+    return hostbuild.load("calib_graph")
 
 
 def c64(a):
@@ -85,7 +65,7 @@ def test_track_elimination_equals_numpy(lib, C):
     for f in range(40):
         w = c64(mask[f] * rng.uniform(0.2, 1.0, size=C))
         H = np.zeros((3 * C, 3 * C))
-        ok = lib.hc_track_block(p(c64(obs[f])), p(w), p(Kinv), p(R), C, p(H))
+        ok = lib.hc_track_block(ptr(c64(obs[f])), ptr(w), ptr(Kinv), ptr(R), C, ptr(H))
         assert ok == (mask[f].sum() >= 2)
         if ok:
             want = restate_block(obs[f], w, K, R)
@@ -107,14 +87,14 @@ def test_pair_cheirality_equals_numpy(lib, C):
         tab = poses[b]["t"] - Rab @ poses[a]["t"]
         E = c64(skew(tab) @ Rab)
         Rs, ts = np.zeros((4, 9)), np.zeros((4, 3))
-        lib.hc_motion_from_essential(p(E), p(Rs), p(ts))
+        lib.hc_motion_from_essential(ptr(E), ptr(Rs), ptr(ts))
         both = np.flatnonzero(mask[:, a] & mask[:, b])[:30]
         for q in range(4):
             Rq, tq = Rs[q].reshape(3, 3), ts[q]
             Pa, Pb = K @ np.hstack([np.eye(3), np.zeros((3, 1))]), K @ np.hstack([Rq, tq[:, None]])
             for f in both:
                 fr = ctypes.c_int(0)
-                got = lib.hc_cheirality(p(c64(K)), p(c64(K)), p(c64(Rq)), p(c64(tq)), *obs[f, a], *obs[f, b], ctypes.byref(fr))
+                got = lib.hc_cheirality(ptr(c64(K)), ptr(c64(K)), ptr(c64(Rq)), ptr(c64(tq)), *obs[f, a], *obs[f, b], ctypes.byref(fr))
                 X = dlt(Pa, Pb, obs[f, a], obs[f, b])
                 cb = -Rq.T @ tq
                 front = X[2] > 0 and (Rq @ X + tq)[2] > 0
@@ -148,13 +128,13 @@ def pair_motions(lib, obs, mask, K, pairs):
         F = eight_point(obs[both, a], obs[both, b])
         E = c64(K.T @ F @ K)
         Rs, ts = np.zeros((4, 9)), np.zeros((4, 3))
-        lib.hc_motion_from_essential(p(E), p(Rs), p(ts))
+        lib.hc_motion_from_essential(ptr(E), ptr(Rs), ptr(ts))
         counts = []
         for q in range(4):
             n = 0
             for f in both:
                 fr = ctypes.c_int(0)
-                lib.hc_cheirality(p(c64(K)), p(c64(K)), p(c64(Rs[q])), p(c64(ts[q])), *obs[f, a], *obs[f, b], ctypes.byref(fr))
+                lib.hc_cheirality(ptr(c64(K)), ptr(c64(K)), ptr(c64(Rs[q])), ptr(c64(ts[q])), *obs[f, a], *obs[f, b], ctypes.byref(fr))
                 n += fr.value
             counts.append(n)
         q = int(np.argmax(counts))
@@ -175,7 +155,7 @@ def test_host_stages_recover_the_true_rig(lib, C):
     w = c64([m[2] for m in mot])
     use = np.ones(len(pairs), dtype=np.uint8)
     R = np.zeros((C, 3, 3)); resid = np.zeros(len(pairs))
-    assert lib.hc_rotation_average(C, len(pairs), p(a), p(b), p(Rab), p(w), 5.0, p(use), p(R), p(resid)) == 1
+    assert lib.hc_rotation_average(C, len(pairs), ptr(a), ptr(b), ptr(Rab), ptr(w), 5.0, ptr(use), ptr(R), ptr(resid)) == 1
     assert use.all() and resid.max() < 1e-4          # degrees through acos: ~1e-6 is its rounding floor near 0
     for c in range(C):
         assert np.abs(R[c] - poses[c]["R"]).max() < 1e-9
@@ -183,7 +163,7 @@ def test_host_stages_recover_the_true_rig(lib, C):
     t = np.zeros((C, 3)); wf = np.zeros(mask.shape)
     f = c64([K[0, 0]] * C)
     init = np.ascontiguousarray(mask, dtype=np.uint8)
-    assert lib.hc_translations(p(c64(obs)), p(init), len(obs), C, p(Kinv), p(c64(R)), p(f), 4, 4.0, p(t), p(wf)) == 1
+    assert lib.hc_translations(ptr(c64(obs)), ptr(init), len(obs), C, ptr(Kinv), ptr(c64(R)), ptr(f), 4, 4.0, ptr(t), ptr(wf)) == 1
     true_t = np.stack([np.asarray(p_["t"]).reshape(3) for p_ in poses])
     true_t = true_t / np.linalg.norm(true_t[1])
     assert np.abs(t - true_t).max() < 1e-9
@@ -202,8 +182,8 @@ def test_rotation_average_drops_a_wrong_pair(lib):
     b = np.array([y for _, y in pairs], dtype=np.int32)
     use = np.ones(len(pairs), dtype=np.uint8)
     R = np.zeros((C, 3, 3)); resid = np.zeros(len(pairs))
-    assert lib.hc_rotation_average(C, len(pairs), p(a), p(b), p(c64(Rab)), p(c64(np.full(len(pairs), 100.0))), 5.0, p(use), p(R),
-                                   p(resid)) == 1
+    assert lib.hc_rotation_average(C, len(pairs), ptr(a), ptr(b), ptr(c64(Rab)), ptr(c64(np.full(len(pairs), 100.0))), 5.0, ptr(use), ptr(R),
+                                   ptr(resid)) == 1
     assert use.sum() == len(pairs) - 1 and not use[bad]
     assert abs(resid[bad] - 30.0) < 1e-6
     for c in range(C):
@@ -211,8 +191,8 @@ def test_rotation_average_drops_a_wrong_pair(lib):
     # a pair graph that the remaining pairs do not connect is refused
     only = np.zeros(len(pairs), dtype=np.uint8)
     only[pairs.index((0, 1))] = 1
-    assert lib.hc_rotation_average(C, len(pairs), p(a), p(b), p(c64(Rab)), p(c64(np.full(len(pairs), 100.0))), 5.0, p(only), p(R),
-                                   p(resid)) == 0
+    assert lib.hc_rotation_average(C, len(pairs), ptr(a), ptr(b), ptr(c64(Rab)), ptr(c64(np.full(len(pairs), 100.0))), 5.0, ptr(only), ptr(R),
+                                   ptr(resid)) == 0
 
 
 def _angle(Ra, Rb):

@@ -5,12 +5,13 @@ import numpy as np
 import pytest
 
 from tests import calib_util as cu
+from tests.hostbuild import ptr
 from tests.test_calib_ransac_on_host import contaminated_pair
 
 
 @pytest.fixture(scope="module")
-def libs(tmp_path_factory):
-    return cu.Libs(tmp_path_factory.mktemp("calib_model"))
+def libs():
+    return cu.Libs()
 
 
 @pytest.mark.parametrize("C", [4, 8, 16])
@@ -80,7 +81,7 @@ def test_ransac_models_scan_equals_selection(libs):
     assert flat[k] == r["count"]
     assert np.array_equal(F.reshape(-1, 3, 3)[k], r["F"])
     mask = np.zeros(len(pts), dtype=np.uint8)
-    libs.rs.hc_inlier_mask(cu.p(cu.c64(r["F"].ravel())), cu.p(cu.c64(pts)), len(pts), 1.0, cu.p(mask))
+    libs.rs.hc_inlier_mask(ptr(cu.c64(r["F"].ravel())), ptr(cu.c64(pts)), len(pts), 1.0, ptr(mask))
     assert np.array_equal(mask.astype(bool), r["mask"])
     assert (cu.ransac_margin(r["F"], pts, 1.0) > 0).all()
 

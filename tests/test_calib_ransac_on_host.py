@@ -3,45 +3,27 @@ the 7-point solver against cv2's FM_7POINT, cv2's fundamental-matrix error and i
 sampler, and the per-pair selection stepped on the host over contaminated pairs."""
 import ctypes
 import importlib
-import os
-import subprocess
 
 import cv2
 import numpy as np
 import pytest
 from scipy import stats
 
+from tests import hostbuild
 from tests.calib_util import eight_point_refit
-from tests.util import ROOT
+from tests.hostbuild import ptr
 
 synth = importlib.import_module("low-cost-mocap_b200.synth")
-HC = os.path.join(ROOT, "tests", "hostcheck")
-_P = ctypes.c_void_p
-_I = ctypes.c_int
 
 
 @pytest.fixture(scope="module")
-def rs(tmp_path_factory):
-    out = str(tmp_path_factory.mktemp("calib_ransac") / "libcalib_ransac_host.so")
-    subprocess.check_call(["g++", "-O2", "-shared", "-fPIC", "-ffp-contract=off", "-o", out,
-                           os.path.join(HC, "calib_ransac_host.cpp"), "-lm"])
-    lib = ctypes.CDLL(out)
-    lib.hc_seven_point.argtypes = [_P, _P, _P]
-    lib.hc_fm_error.argtypes = [_P, _P, _I, _P]
-    lib.hc_inlier_mask.argtypes = [_P, _P, _I, ctypes.c_double, _P]
-    lib.hc_draw7.argtypes = [ctypes.c_uint64, _I, _I, _I, _I, _I, _P]
-    lib.hc_has_collinear.argtypes = [_P]
-    lib.hc_ransac_select.argtypes = [_P, _I, _I, _I, ctypes.c_uint64, ctypes.c_double, _P, _P, _P]
-    return lib
-
-
-def _p(a):
-    return a.ctypes.data_as(_P)
+def rs():
+    return hostbuild.load("calib_ransac")
 
 
 def _draw(rs, seed, p, h0, count, m, attempt=0):
     idx = np.zeros((count, 7), dtype=np.int32)
-    rs.hc_draw7(seed, p, h0, count, attempt, m, _p(idx))
+    rs.hc_draw7(seed, p, h0, count, attempt, m, ptr(idx))
     return idx
 
 
@@ -96,8 +78,8 @@ def test_seven_point_matches_cv2(rs):
             continue
         tried += 1
         out = np.zeros(27)
-        n = rs.hc_seven_point(_p(np.ascontiguousarray(a.astype(np.float64).ravel())),
-                              _p(np.ascontiguousarray(b.astype(np.float64).ravel())), _p(out))
+        n = rs.hc_seven_point(ptr(np.ascontiguousarray(a.astype(np.float64).ravel())),
+                              ptr(np.ascontiguousarray(b.astype(np.float64).ravel())), ptr(out))
         assert n == len(ref)
         roots.add(n)
         for k in range(n):
@@ -112,11 +94,11 @@ def test_seven_point_degenerate_samples_give_no_model(rs):
     rng = np.random.default_rng(4)
     b = rng.uniform(0, 480, 14)
     out = np.zeros(27)
-    assert rs.hc_seven_point(_p(np.full(14, 100.0)), _p(b), _p(out)) == 0
+    assert rs.hc_seven_point(ptr(np.full(14, 100.0)), ptr(b), ptr(out)) == 0
     t = np.sort(rng.uniform(0, 1, 7))
     line = np.ascontiguousarray(np.c_[100 + 300 * t, 50 + 200 * t].ravel())
-    assert rs.hc_seven_point(_p(line), _p(b), _p(out)) == 0
-    assert rs.hc_has_collinear(_p(line)) == 1
+    assert rs.hc_seven_point(ptr(line), ptr(b), ptr(out)) == 0
+    assert rs.hc_has_collinear(ptr(line)) == 1
 
 
 def test_fm_error_matches_numpy(rs):
@@ -124,7 +106,7 @@ def test_fm_error_matches_numpy(rs):
     F = rng.normal(size=9)
     pts = np.ascontiguousarray(rng.uniform(0, 640, (1000, 4)))
     err = np.zeros(1000)
-    rs.hc_fm_error(_p(F), _p(pts), 1000, _p(err))
+    rs.hc_fm_error(ptr(F), ptr(pts), 1000, ptr(err))
     Fm = F.reshape(3, 3)
     x1 = np.c_[pts[:, :2], np.ones(1000)]
     x2 = np.c_[pts[:, 2:], np.ones(1000)]
@@ -144,7 +126,7 @@ def test_inlier_mask_agrees_with_cv2(rs, frac):
         F, mask = cv2.findFundamentalMat(a, b, cv2.FM_RANSAC, 1, 0.99999)
         pts = np.ascontiguousarray(np.c_[a, b].astype(np.float64))
         mine = np.zeros(len(a), dtype=np.uint8)
-        rs.hc_inlier_mask(_p(np.ascontiguousarray(F.ravel())), _p(pts), len(a), 1.0, _p(mine))
+        rs.hc_inlier_mask(ptr(np.ascontiguousarray(F.ravel())), ptr(pts), len(a), 1.0, ptr(mine))
         assert (mine == mask.ravel()).mean() >= 0.99
 
 
@@ -182,7 +164,7 @@ def test_host_selection_recovers_rotation(rs, frac):
         F = np.zeros(9)
         mask = np.zeros(len(x1), dtype=np.uint8)
         cnt = ctypes.c_int()
-        assert rs.hc_ransac_select(_p(pts), len(x1), 0, 2048, 0, 1.0, _p(F), _p(mask), ctypes.byref(cnt)) == 1
+        assert rs.hc_ransac_select(ptr(pts), len(x1), 0, 2048, 0, 1.0, ptr(F), ptr(mask), ctypes.byref(cnt)) == 1
         inl = mask.astype(bool)
         assert cnt.value == inl.sum()
         assert inl[~bad].mean() >= 0.75 and (inl[bad].mean() if bad.any() else 0) <= 0.05

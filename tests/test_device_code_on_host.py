@@ -5,36 +5,31 @@ moments, ranking -- is checked against the reference's golden vectors and cv2 on
 (The GPU parity tests in test_parity_gpu.py run the same code on the device through the C ABI.)"""
 import ctypes
 import os
+import shutil
 import subprocess
 
 import numpy as np
 import pytest
 
+from tests import hostbuild
+from tests.hostbuild import HC, ptr
 from tests.util import ROOT, load_golden
 
 PIPE_CASES = ["pipe_c2_m1", "pipe_c4_m4", "pipe_c8_m16"]
 
 pytestmark = pytest.mark.timeout(300)        # a divergent barrier in the device code shows up as a deadlock here
 
-HC = os.path.join(ROOT, "tests", "hostcheck")
-CUDA_INC = os.path.join(os.environ.get("CUDA_HOME", "/usr/local/cuda"), "include")
-
 
 @pytest.fixture(scope="module")
 def blob_emu():
-    src = os.path.join(HC, "blob_emu_host.cpp")
-    out = os.path.join(HC, "libblob_emu.so")
-    subprocess.check_call(["g++", "-std=c++20", "-O2", "-shared", "-fPIC", "-pthread", "-I" + CUDA_INC, "-Wno-attributes",
-                           "-fno-strict-aliasing", "-o", out, src])
-    lib = ctypes.CDLL(out)
+    lib = hostbuild.load("blob_emu")
 
     def detect(img, threshold=51, max_blobs=64, E=1024, force_cta=0, seed=1):
         img = np.ascontiguousarray(img, dtype=np.uint8)
         H, W = img.shape
         xy = np.zeros((max_blobs, 2), np.int32); n = np.zeros(1, np.int32)
         mom = np.zeros((max_blobs, 4), np.int64); fl = np.zeros(1, np.int32)
-        p = lambda a: a.ctypes.data_as(ctypes.c_void_p)
-        rc = lib.hc_blob_detect(p(img), W, H, int(threshold), max_blobs, E, force_cta, seed, p(xy), p(n), p(mom), p(fl))
+        rc = lib.hc_blob_detect(ptr(img), W, H, int(threshold), max_blobs, E, force_cta, seed, ptr(xy), ptr(n), ptr(mom), ptr(fl))
         assert rc >= 0, rc
         return {"path": rc, "n": int(n[0]), "xy": xy[:n[0]].copy(), "mom": mom[:n[0]].copy(), "flags": int(fl[0])}
     return detect
@@ -139,11 +134,7 @@ ERR_RTOL = 1e-9
 
 @pytest.fixture(scope="module")
 def match_emu():
-    src = os.path.join(HC, "match_emu_host.cpp")
-    out = os.path.join(HC, "libmatch_emu.so")
-    subprocess.check_call(["g++", "-std=c++20", "-O2", "-shared", "-fPIC", "-pthread", "-I" + CUDA_INC, "-Wno-attributes",
-                           "-fno-strict-aliasing", "-o", out, src])
-    lib = ctypes.CDLL(out)
+    lib = hostbuild.load("match_emu")
 
     def match(K, R, t, blob_xy, blob_n, max_roots=128, max_cands=8, max_groups=4096):
         C = len(R)
@@ -154,9 +145,8 @@ def match_emu():
         xy = np.ascontiguousarray(blob_xy, dtype=np.int32); n = np.ascontiguousarray(blob_n, dtype=np.int32)
         obj = np.zeros((B, max_roots, 3)); err = np.zeros((B, max_roots))
         k = np.zeros(B, np.int32); fl = np.zeros(B, np.int32)
-        p = lambda a: a.ctypes.data_as(ctypes.c_void_p)
-        assert lib.hc_match_triangulate(p(K), p(R), p(t), C, p(xy), p(n), B, MB, max_roots, max_cands, ctypes.c_uint(max_groups),
-                                        p(obj), p(err), p(k), p(fl)) == 0
+        assert lib.hc_match_triangulate(ptr(K), ptr(R), ptr(t), C, ptr(xy), ptr(n), B, MB, max_roots, max_cands, ctypes.c_uint(max_groups),
+                                        ptr(obj), ptr(err), ptr(k), ptr(fl)) == 0
         return {"obj": obj, "err": err, "n": k, "flags": fl}
 
     def chunked(K, R, t, blob_xy, blob_n, chunk, item_cap, n_ctas=3, max_roots=128, max_cands=8, max_groups=4096):
@@ -169,10 +159,9 @@ def match_emu():
         xy = np.ascontiguousarray(blob_xy, dtype=np.int32); n = np.ascontiguousarray(blob_n, dtype=np.int32)
         obj = np.zeros((B, max_roots, 3)); err = np.zeros((B, max_roots))
         k = np.zeros(B, np.int32); fl = np.zeros(B, np.int32); txy = np.zeros((B, max_roots, C, 2), np.int32); stats = np.zeros(3, np.int64)
-        p = lambda a: a.ctypes.data_as(ctypes.c_void_p)
-        assert lib.hc_match_triangulate_chunked(p(K), p(R), p(t), C, p(xy), p(n), B, MB, max_roots, max_cands, ctypes.c_uint(max_groups),
+        assert lib.hc_match_triangulate_chunked(ptr(K), ptr(R), ptr(t), C, ptr(xy), ptr(n), B, MB, max_roots, max_cands, ctypes.c_uint(max_groups),
                                                 ctypes.c_uint(chunk), ctypes.c_uint(item_cap), n_ctas,
-                                                p(obj), p(err), p(k), p(fl), p(txy), p(stats)) == 0
+                                                ptr(obj), ptr(err), ptr(k), ptr(fl), ptr(txy), ptr(stats)) == 0
         return {"obj": obj, "err": err, "n": k, "flags": fl, "track_xy": txy, "items": int(stats[0]), "claimed": int(stats[1]), "armed": int(stats[2])}
     match.chunked = chunked
     return match
@@ -268,11 +257,7 @@ def test_matcher_device_code_capacity_flags(match_emu):
 # ------------------------------------------------------------------------- the single-pass pipeline kernel
 @pytest.fixture(scope="module")
 def fused_emu():
-    src = os.path.join(HC, "fused_emu_host.cpp")
-    out = os.path.join(HC, "libfused_emu.so")
-    subprocess.check_call(["g++", "-std=c++20", "-O2", "-shared", "-fPIC", "-pthread", "-I" + CUDA_INC, "-Wno-attributes",
-                           "-fno-strict-aliasing", "-o", out, src])
-    lib = ctypes.CDLL(out)
+    lib = hostbuild.load("fused_emu")
 
     def run(frames, K, R, t, threshold=51, max_blobs=64, E=1024, max_roots=128, max_cands=8, max_groups=4096, n_warps=8, runs=2):
         frames = np.ascontiguousarray(frames, dtype=np.uint8)
@@ -283,9 +268,8 @@ def fused_emu():
         obj = np.zeros((B, max_roots, 3)); err = np.zeros((B, max_roots)); k = np.zeros(B, np.int32); fl = np.zeros(B, np.int32)
         bxy = np.zeros((B * C, max_blobs, 2), np.int32); bn = np.zeros(B * C, np.int32)
         iw = np.zeros(B * C, np.uint32); sw = np.zeros(B, np.uint32); cnt = np.zeros(4, np.int64)
-        p = lambda a: a.ctypes.data_as(ctypes.c_void_p)
-        rc = lib.hc_pipeline_fused(p(frames), B, C, W, H, int(threshold), p(K), p(R), p(t), max_blobs, E, max_roots, max_cands,
-                                   ctypes.c_uint(max_groups), n_warps, runs, p(obj), p(err), p(k), p(fl), p(bxy), p(bn), p(iw), p(sw), p(cnt), channels)
+        rc = lib.hc_pipeline_fused(ptr(frames), B, C, W, H, int(threshold), ptr(K), ptr(R), ptr(t), max_blobs, E, max_roots, max_cands,
+                                   ctypes.c_uint(max_groups), n_warps, runs, ptr(obj), ptr(err), ptr(k), ptr(fl), ptr(bxy), ptr(bn), ptr(iw), ptr(sw), ptr(cnt), channels)
         assert rc == 0
         return {"obj": obj, "err": err, "n": k, "flags": fl, "blob_xy": bxy.reshape(B, C, max_blobs, 2), "blob_n": bn.reshape(B, C),
                 "deferred_images": iw[:cnt[0]].tolist(), "deferred_sets": sw[:cnt[1]].tolist(), "dirty_scratch": int(cnt[2])}
@@ -370,21 +354,10 @@ def test_device_code_has_no_unintended_data_races(tmp_path):
     fence between warps (or lanes) is a reportable data race.  The union-find of the blob reduce races BY DESIGN
     (lock-free path halving + atomicMin, blob_device.cuh) and is suppressed; nothing else may be reported, on
     light frame-sets and on the deferral path."""
-    import shutil
-    tsan = subprocess.run(["gcc", "-print-file-name=libtsan.so"], capture_output=True, text=True).stdout.strip()
-    if not tsan or not os.path.isabs(tsan) or not os.path.exists(tsan):
-        pytest.skip("libtsan not available")
-    libs = {}
-    for name in ("fused", "blob", "match"):
-        libs[name] = str(tmp_path / f"lib{name}_tsan.so")
-        subprocess.check_call(["g++", "-std=c++20", "-O1", "-g", "-fsanitize=thread", "-shared", "-fPIC", "-pthread", "-I" + CUDA_INC,
-                               "-Wno-attributes", "-Wno-tsan", "-fno-strict-aliasing", "-o", libs[name], os.path.join(HC, f"{name}_emu_host.cpp")])
-    lib = libs["fused"]
-    supp = tmp_path / "supp.txt"
-    supp.write_text("race:uf_find\nrace:uf_unite\nrace:atomicMin\n")
-    env = dict(os.environ, LD_PRELOAD=tsan, TSAN_OPTIONS=f"report_signal_unsafe=0 history_size=4 exitcode=0 suppressions={supp}")
+    env = hostbuild.tsan_env(tmp_path, ["race:uf_find", "race:uf_unite", "race:atomicMin"])
+    libs = {name: hostbuild.build(f"{name}_emu", tsan=True) for name in ("fused", "blob", "match")}
     for extra in ([], ["crowded"]):
-        r = subprocess.run([shutil.which("python") or "python", os.path.join(HC, "tsan_fused_run.py"), ROOT, lib, "pipe_c4_m4"] + extra,
+        r = subprocess.run([shutil.which("python") or "python", os.path.join(HC, "tsan_fused_run.py"), ROOT, libs["fused"], "pipe_c4_m4"] + extra,
                            capture_output=True, text=True, env=env, timeout=280)
         out = r.stdout + r.stderr
         assert "RESULT 0" in out, out[-2000:]
@@ -517,22 +490,14 @@ def test_single_pass_kernel_on_host_defers_exactly_the_holed_images(fused_emu, b
 # ---------------------------------------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
 def ba_emu():
-    out = os.path.join(HC, "libba_dev_emu.so")
-    subprocess.check_call(["g++", "-std=c++20", "-O2", "-shared", "-fPIC", "-pthread", "-I" + CUDA_INC, "-Wno-attributes",
-                           "-fno-strict-aliasing", "-o", out, os.path.join(HC, "ba_dev_emu_host.cpp")])
-    model = os.path.join(HC, "libba_host.so")
-    subprocess.check_call(["g++", "-O2", "-shared", "-fPIC", "-o", model, os.path.join(HC, "ba_host.cpp"), "-lm"])
-    emu, host = ctypes.CDLL(out), ctypes.CDLL(model)
-    emu.hc_ba_solve_dev.argtypes = [ctypes.c_void_p] * 2 + [ctypes.c_int] * 2 + [ctypes.c_void_p] * 3 + [ctypes.c_double] + [ctypes.c_int] * 6 + [ctypes.c_void_p]
-    host.hc_bundle_adjust.argtypes = [ctypes.c_void_p] * 2 + [ctypes.c_int] * 2 + [ctypes.c_void_p] * 3 + [ctypes.c_double, ctypes.c_int, ctypes.c_void_p, ctypes.c_int]
-    p = lambda a: a.ctypes.data_as(ctypes.c_void_p)
+    emu, host = hostbuild.load("ba_dev_emu"), hostbuild.load("ba")
 
     def solve(obs, mask, K, R, t, prefit, n_ctas, n_threads, jac_mode=1, max_nfev=0):
         C = mask.shape[1]
         obs = np.ascontiguousarray(obs, np.float64); mask = np.ascontiguousarray(mask, np.uint8)
         Ks = np.ascontiguousarray(np.stack([K] * C)); R = np.ascontiguousarray(R.copy()); t = np.ascontiguousarray(t.copy())
         rep = np.zeros(13)
-        assert emu.hc_ba_solve_dev(p(obs), p(mask), obs.shape[0], C, p(Ks), p(R), p(t), 1e-2, max_nfev, jac_mode, int(prefit), 50, n_ctas, n_threads, p(rep)) == 0
+        assert emu.hc_ba_solve_dev(ptr(obs), ptr(mask), obs.shape[0], C, ptr(Ks), ptr(R), ptr(t), 1e-2, max_nfev, jac_mode, int(prefit), 50, n_ctas, n_threads, ptr(rep)) == 0
         keys = ["cost_initial", "cost_final", "optimality", "n_iterations", "n_fev", "status", "n_residuals", "prefit_cost_initial",
                 "prefit_cost_final", "prefit_iterations", "smem", "n_tr_solves", "n_tr_newton"]
         return R, t, dict(zip(keys, rep))
@@ -542,7 +507,7 @@ def ba_emu():
         obs = np.ascontiguousarray(obs, np.float64); mask = np.ascontiguousarray(mask, np.uint8)
         Ks = np.ascontiguousarray(np.stack([K] * C)); R = np.ascontiguousarray(R.copy()); t = np.ascontiguousarray(t.copy())
         rep = np.zeros(7)
-        assert host.hc_bundle_adjust(p(obs), p(mask), obs.shape[0], C, p(Ks), p(R), p(t), 1e-2, 0, p(rep), jac_mode) == 0
+        assert host.hc_bundle_adjust(ptr(obs), ptr(mask), obs.shape[0], C, ptr(Ks), ptr(R), ptr(t), 1e-2, 0, ptr(rep), jac_mode) == 0
         return R, t, dict(zip(["cost_initial", "cost_final", "optimality", "n_iterations", "n_fev", "status", "n_jev"], rep))
     return solve, model_solve
 

@@ -47,8 +47,8 @@ def torch():
 
 
 @pytest.fixture(scope="module")
-def libs(tmp_path_factory):
-    return cu.Libs(tmp_path_factory.mktemp("calib_vs_model"))
+def libs():
+    return cu.Libs()
 
 
 def _ctx(C, K):

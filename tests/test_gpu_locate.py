@@ -9,7 +9,8 @@ import importlib
 import numpy as np
 import pytest
 
-from tests.locate_util import (GUARD, MAX_POINTS, SENTINEL_F, SENTINEL_I, bits, build_locate_host, check_guards, compare_to_oracle, count_cases,
+from tests import hostbuild
+from tests.locate_util import (GUARD, MAX_POINTS, SENTINEL_F, SENTINEL_I, bits, check_guards, compare_to_oracle, count_cases,
                                edge_scenes, equal_but_heading, fold_allowed, fuzz_scenes, guarded_outputs, host_locate_batch,
                                large_scenes, oracle, pack, small_scenes)
 
@@ -28,8 +29,8 @@ def torch():
 
 
 @pytest.fixture(scope="module")
-def lib(tmp_path_factory):
-    return build_locate_host(tmp_path_factory.mktemp("locate"))
+def lib():
+    return hostbuild.load("locate")
 
 
 def _ctx(R):

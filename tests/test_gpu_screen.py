@@ -7,7 +7,8 @@ import importlib
 import numpy as np
 import pytest
 
-from tests.screen_util import build_screen_host, contaminated_tracks, host_screen, poses_arrays, screen_inputs
+from tests import hostbuild
+from tests.screen_util import contaminated_tracks, host_screen, poses_arrays, screen_inputs
 
 pytestmark = pytest.mark.gpu
 
@@ -27,8 +28,8 @@ def torch():
 
 
 @pytest.fixture(scope="module")
-def lib(tmp_path_factory):
-    return build_screen_host(tmp_path_factory.mktemp("screen"))
+def lib():
+    return hostbuild.load("screen")
 
 
 def _ctx(C, K, poses=None):

@@ -8,7 +8,8 @@ import importlib
 import numpy as np
 import pytest
 
-from tests.track_util import (build_track_host, golden_stream, host_run, load_golden, make_stream, objects_of, run_batches,
+from tests import hostbuild
+from tests.track_util import (golden_stream, host_run, load_golden, make_stream, objects_of, run_batches,
                               run_oracle)
 
 pytestmark = pytest.mark.gpu
@@ -29,8 +30,8 @@ def torch():
 
 
 @pytest.fixture(scope="module")
-def lib(tmp_path_factory):
-    return build_track_host(tmp_path_factory.mktemp("track"))
+def lib():
+    return hostbuild.load("track")
 
 
 @pytest.fixture(scope="module")

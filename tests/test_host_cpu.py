@@ -11,6 +11,8 @@ import sys
 import numpy as np
 import pytest
 
+from tests import hostbuild
+from tests.hostbuild import ptr
 from tests.util import ROOT, load_golden
 
 pkg = importlib.import_module("low-cost-mocap_b200")
@@ -121,12 +123,7 @@ def test_track_all_gather_gloo_world2(tmp_path):
 
 @pytest.fixture(scope="module")
 def geom_host():
-    src = os.path.join(ROOT, "tests", "hostcheck", "geom_host.cpp")
-    out = os.path.join(ROOT, "tests", "hostcheck", "libgeom_host.so")
-    if not os.path.exists(out) or os.path.getmtime(out) < max(os.path.getmtime(src), os.path.getmtime(
-            os.path.join(ROOT, "low-cost-mocap_b200", "csrc", "geom.cuh"))):
-        subprocess.check_call(["g++", "-O2", "-shared", "-fPIC", "-ffp-contract=off", "-o", out, src, "-lm"])
-    return ctypes.CDLL(out)
+    return hostbuild.load("geom")
 
 
 @pytest.mark.parametrize("name", ["tri_c4", "tri_c8", "tri_c16"])
@@ -143,8 +140,7 @@ def test_geometry_code_matches_golden_on_host(geom_host, name):
             Pkc[k, c] = (K @ np.c_[R[c], t[c]]).ravel()
     K4 = np.tile(np.array([K[0, 0], K[1, 1], K[0, 2], K[1, 2]]), (C, 1))
     X = np.zeros((n, 3)); err = np.zeros(n); valid = np.zeros(n, np.uint8)
-    p = lambda a: a.ctypes.data_as(ctypes.c_void_p)
-    geom_host.hc_triangulate(p(obs), p(mask), n, C, p(Pkc), p(R), p(t), p(K4), p(X), p(err), p(valid))
+    geom_host.hc_triangulate(ptr(obs), ptr(mask), n, C, ptr(Pkc), ptr(R), ptr(t), ptr(K4), ptr(X), ptr(err), ptr(valid))
     assert valid.all()
     assert np.abs(X - z["X"]).max() < 1e-9
     assert np.array_equal(err, z["err"])
@@ -157,7 +153,6 @@ def test_dlt_null_vector_at_near_degenerate_geometry_on_host(geom_host):
     Jacobi solver agree to 1e-12 wherever the fast path settles, and the degenerate cases really send points to Jacobi."""
     pytest.importorskip("mpmath")
     from tests.util import dlt_cases, dlt_matrix, exact_dlt_point
-    p = lambda a: a.ctypes.data_as(ctypes.c_void_p)
     fallbacks = {}
     for name, Ks, poses, obs, mask in dlt_cases():
         n, C = mask.shape
@@ -168,7 +163,7 @@ def test_dlt_null_vector_at_near_degenerate_geometry_on_host(geom_host):
                 Pkc[k, c] = (Ks[k] @ np.c_[R[c], t[c]]).ravel()
         K4 = np.array([[K[0, 0], K[1, 1], K[0, 2], K[1, 2]] for K in Ks])
         X = np.zeros((n, 3)); err = np.zeros(n); valid = np.zeros(n, np.uint8)
-        geom_host.hc_triangulate(p(np.ascontiguousarray(obs)), p(mask), n, C, p(Pkc), p(R), p(t), p(K4), p(X), p(err), p(valid))
+        geom_host.hc_triangulate(ptr(np.ascontiguousarray(obs)), ptr(mask), n, C, ptr(Pkc), ptr(R), ptr(t), ptr(K4), ptr(X), ptr(err), ptr(valid))
         assert valid.all()
         Bs = np.zeros((n, 10))
         checked = 0
@@ -183,7 +178,7 @@ def test_dlt_null_vector_at_near_degenerate_geometry_on_host(geom_host):
             assert np.abs(X[f] - Xe).max() <= 1e-11 * max(1.0, np.abs(Xe).max()), (name, f, X[f], Xe)
         assert checked >= n - 2, name
         worst, fb = ctypes.c_double(), ctypes.c_int()
-        geom_host.hc_null_vector_compare(p(Bs), n, ctypes.byref(worst), ctypes.byref(fb))
+        geom_host.hc_null_vector_compare(ptr(Bs), n, ctypes.byref(worst), ctypes.byref(fb))
         assert worst.value <= 1e-12, (name, worst.value)
         fallbacks[name] = fb.value
     assert fallbacks["baseline_1cm"] > 0 and fallbacks["near_baseline_epipole"] > 0, fallbacks
@@ -203,10 +198,7 @@ def test_header_is_plain_c_and_example_links(built_lib, tmp_path):
 
 @pytest.fixture(scope="module")
 def ba_host():
-    src = os.path.join(ROOT, "tests", "hostcheck", "ba_host.cpp")
-    out = os.path.join(ROOT, "tests", "hostcheck", "libba_host.so")
-    subprocess.check_call(["g++", "-O2", "-shared", "-fPIC", "-ffp-contract=off", "-o", out, src, "-lm"])
-    return ctypes.CDLL(out)
+    return hostbuild.load("ba")
 
 
 def test_trust_region_control_equals_scipy_on_a_smooth_problem(ba_host):
@@ -218,13 +210,11 @@ def test_trust_region_control_equals_scipy_on_a_smooth_problem(ba_host):
     t = np.linspace(0, 4, 40)
     y = 2.5 * np.exp(-1.3 * t) + 0.5 + rng.normal(0, 0.05, 40)
     y[::7] += 3.0                                    # outliers for the Cauchy loss
-    p = lambda a: a.ctypes.data_as(ctypes.c_void_p)
-    ba_host.hc_trf_expfit.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_double, ctypes.c_void_p]
     for ftol in (1e-2, 1e-8):
         x0 = np.array([1.0, 0.5, 0.0, 7.0])
         ref = least_squares(lambda x: x[0] * np.exp(-x[1] * t) + x[2] - y, x0, loss="cauchy", ftol=ftol)
         x = x0.copy(); rep = np.zeros(7)
-        assert ba_host.hc_trf_expfit(p(t), p(y), 40, p(x), ftol, p(rep)) == 0
+        assert ba_host.hc_trf_expfit(ptr(t), ptr(y), 40, ptr(x), ftol, ptr(rep)) == 0
         assert np.allclose(x, ref.x, rtol=1e-6, atol=1e-8)
         assert abs(rep[1] - ref.cost) < 1e-9 * max(1.0, ref.cost)
         assert int(rep[4]) == ref.nfev and int(rep[5]) == ref.status
@@ -239,19 +229,14 @@ def test_ba_host_model_reaches_reference_quality(ba_host):
     K = np.ascontiguousarray(np.tile(z["K"].reshape(1, 9), (C, 1)))
     R = np.ascontiguousarray(z["R_start"].copy()); t = np.ascontiguousarray(z["t_start"].copy())
     rep = np.zeros(7)
-    p = lambda a: a.ctypes.data_as(ctypes.c_void_p)
-    ba_host.hc_bundle_adjust.argtypes = [ctypes.c_void_p] * 2 + [ctypes.c_int] * 2 + [ctypes.c_void_p] * 3 + [ctypes.c_double, ctypes.c_int, ctypes.c_void_p, ctypes.c_int]
-    assert ba_host.hc_bundle_adjust(p(obs), p(mask), obs.shape[0], C, p(K), p(R), p(t), 1e-2, 0, p(rep), 1) == 0
+    assert ba_host.hc_bundle_adjust(ptr(obs), ptr(mask), obs.shape[0], C, ptr(K), ptr(R), ptr(t), 1e-2, 0, ptr(rep), 1) == 0
     assert abs(rep[0] - float(z["cost0"])) < 1e-3 * float(z["cost0"])
     assert rep[1] < 0.5 * rep[0] and int(rep[5]) in (2, 3, 4)
 
 
 @pytest.fixture(scope="module")
 def preproc_host():
-    src = os.path.join(ROOT, "tests", "hostcheck", "preproc_host.cpp")
-    out = os.path.join(ROOT, "tests", "hostcheck", "libpreproc_host.so")
-    subprocess.check_call(["g++", "-O2", "-shared", "-fPIC", "-fno-strict-aliasing", "-o", out, src])
-    return ctypes.CDLL(out)
+    return hostbuild.load("preproc")
 
 
 @pytest.mark.parametrize("S,in_h,rot,word_stores,n_threads", [(320, 240, 0, 1, 256), (320, 240, 2, 0, 256), (200, 150, 2, 1, 96),
@@ -272,7 +257,6 @@ def test_preprocess_tile_stages_equal_cv2_chain_on_host(preproc_host, S, in_h, r
     rng = np.random.default_rng(S + rot)
     frames = np.stack([rng.integers(0, 256, size=(in_h, S, 3), dtype=np.uint8), np.full((in_h, S, 3), 255, dtype=np.uint8),
                        (rng.integers(0, 2, size=(in_h, S, 3)) * 255).astype(np.uint8)])
-    p = lambda a: a.ctypes.data_as(ctypes.c_void_p) if a is not None else None
     ws = word_stores if S % 4 == 0 else 0
     want = np.stack([port.preprocess(raw, 0, dist, rot) for raw in frames])
     want_gray = np.stack([cv2.cvtColor(w, cv2.COLOR_RGB2GRAY) for w in want])        # what _find_dot thresholds (helpers.py:144)
@@ -283,11 +267,11 @@ def test_preprocess_tile_stages_equal_cv2_chain_on_host(preproc_host, S, in_h, r
             raw = np.ascontiguousarray(frames[first:first + n])
             got = np.full((n, S, S, 3), 7, dtype=np.uint8)
             gray = np.full((n, S, S), 7, dtype=np.uint8)
-            preproc_host.hc_preprocess(p(raw), n, S, in_h, S, rot, p(m1), p(m2), p(got), p(gray), ws, n_threads)
+            preproc_host.hc_preprocess(ptr(raw), n, S, in_h, S, rot, ptr(m1), ptr(m2), ptr(got), ptr(gray), ws, n_threads)
             assert np.array_equal(got, want[first:first + n]), int((got != want[first:first + n]).sum())
             assert np.array_equal(gray, want_gray[first:first + n])
             only_gray = np.zeros((n, S, S), dtype=np.uint8)
-            preproc_host.hc_preprocess(p(raw), n, S, in_h, S, rot, p(m1), p(m2), None, p(only_gray), ws, n_threads)
+            preproc_host.hc_preprocess(ptr(raw), n, S, in_h, S, rot, ptr(m1), ptr(m2), None, ptr(only_gray), ws, n_threads)
             assert np.array_equal(only_gray, gray)
 
 
@@ -299,7 +283,6 @@ def test_preprocess_tile_stages_fuzz_on_host(preproc_host):
     from oracle.ref_port import RefPort
     from tests.preproc_util import fuzz_camera
     rng = np.random.default_rng(2024)
-    p = lambda a: a.ctypes.data_as(ctypes.c_void_p) if a is not None else None
     for case in range(24):
         S = int(rng.integers(34, 150))
         in_h = int(rng.integers(1, S - 15)) if case % 4 else S - 16
@@ -312,7 +295,7 @@ def test_preprocess_tile_stages_fuzz_on_host(preproc_host):
         want = np.stack([port.preprocess(r, 0, dist, rot) for r in raw])
         got = np.full((2, S, S, 3), 9, dtype=np.uint8)
         gray = np.full((2, S, S), 9, dtype=np.uint8)
-        preproc_host.hc_preprocess(p(raw), 2, S, in_h, S, rot, p(m1), p(m2), p(got), p(gray), 1 if S % 4 == 0 else 0,
+        preproc_host.hc_preprocess(ptr(raw), 2, S, in_h, S, rot, ptr(m1), ptr(m2), ptr(got), ptr(gray), 1 if S % 4 == 0 else 0,
                                    int(rng.choice([32, 96, 256])))
         assert np.array_equal(got, want), (case, S, in_h, rot, int((got != want).sum()))
         assert np.array_equal(gray, np.stack([cv2.cvtColor(w, cv2.COLOR_RGB2GRAY) for w in want])), (case, S, in_h, rot)

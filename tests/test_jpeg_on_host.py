@@ -2,41 +2,23 @@
 recorded bytes of tests/golden/jpeg_cv2.npz; the host build of csrc/jpeg.cuh (the kernels' step code) against the model
 stage by stage -- colour conversion and downsampling, the DCT and quantisation, bit counts, packing and stuffing on
 random and extreme coefficient blocks -- and whole; install_into(stream=True) on stand-ins."""
-import ctypes
 import importlib
-import os
-import subprocess
 
 import cv2
 import numpy as np
 import pytest
 
+from tests import hostbuild
 from tests import jpeg_util as J
-from tests.live_util import ROOT
+from tests.hostbuild import ptr
 
 api = importlib.import_module("low-cost-mocap_b200.api")
 pkg = importlib.import_module("low-cost-mocap_b200")
-P, I, U64 = ctypes.c_void_p, ctypes.c_int, ctypes.c_uint64
 
 
 @pytest.fixture(scope="module")
-def lib(tmp_path_factory):
-    out = os.path.join(str(tmp_path_factory.mktemp("jpeg")), "libjpeg_host.so")
-    subprocess.check_call(["g++", "-O2", "-shared", "-fPIC", "-ffp-contract=off", "-std=c++17", "-o", out,
-                           os.path.join(ROOT, "tests", "hostcheck", "jpeg_host.cpp")])
-    lib = ctypes.CDLL(out)
-    for name, res, args in (("hc_tables_size", I, []), ("hc_header", None, [I, I, I, P]), ("hc_bound", U64, [I, I]),
-                            ("hc_ycc", None, [I, P, P]), ("hc_samples", None, [P, I, I, I, P]), ("hc_fdct", None, [I, P, P]),
-                            ("hc_quantize", None, [I, I, P, P, P]), ("hc_block_bits", None, [I, P, P, P, P, P]),
-                            ("hc_pack", None, [I, P, P, P, P, U64, P]), ("hc_stuff", U64, [P, U64, I, P]),
-                            ("hc_encode", ctypes.c_int64, [P, I, I, I, I, P, U64])):
-        fn = getattr(lib, name)
-        fn.restype, fn.argtypes = res, args
-    return lib
-
-
-def _p(a):
-    return a.ctypes.data_as(P)
+def lib():
+    return hostbuild.load("jpeg")
 
 
 def _i32(a):
@@ -80,7 +62,7 @@ def test_header_is_cv2s():
 def test_tables_and_header(lib):
     for q in (1, 10, 50, 75, 95, 100):
         h = np.zeros(623, np.uint8)
-        lib.hc_header(1280, 320, q, _p(h))
+        lib.hc_header(1280, 320, q, ptr(h))
         assert bytes(h) == J.header(1280, 320, q), q
     assert lib.hc_bound(16, 16) == 623 + 2 * (9960 // 8) + 2
 
@@ -90,7 +72,7 @@ def test_colour_conversion(lib):
     px = np.concatenate([rng.integers(0, 256, (20000, 3)), np.array(np.meshgrid([0, 1, 127, 128, 254, 255], [0, 255], [0, 128, 255])).reshape(3, -1).T])
     px = np.ascontiguousarray(px, np.uint8)
     out = np.zeros((len(px), 3), np.int32)
-    lib.hc_ycc(len(px), _p(px), _p(out))
+    lib.hc_ycc(len(px), ptr(px), ptr(out))
     assert np.array_equal(out, np.stack(J.rgb_ycc(px), -1))
 
 
@@ -104,7 +86,7 @@ def test_samples_colour_and_downsampling(lib, h, w, tiles):
     W = tiles * w
     mh, mw = -(-h // 16), -(-W // 16)
     got = np.zeros((mh * mw, 6, 64), np.int32)
-    lib.hc_samples(_p(frames), tiles, w, h, _p(got))
+    lib.hc_samples(ptr(frames), tiles, w, h, ptr(got))
     Y, Cb, Cr = J.planes(img)
     got = got.reshape(mh, mw, 6, 8, 8)
     hb, wb = -(-h // 8), -(-W // 8)
@@ -128,14 +110,14 @@ def test_fdct_and_quantisation(lib):
     rng = np.random.default_rng(1)
     s = _sample_blocks(rng, 5000)
     d = np.zeros_like(s)
-    lib.hc_fdct(len(s), _p(s), _p(d))
+    lib.hc_fdct(len(s), ptr(s), ptr(d))
     want = J.fdct_islow(s.reshape(-1, 8, 8)).reshape(-1, 64)
     assert np.array_equal(d, want)
     assert np.abs(d).max() >= 8000                   # the extremes reach the DC's range
     tabs = _i32(rng.integers(0, 2, len(d)))
     for q in (1, 10, 50, 75, 95, 100):
         zz = np.zeros(d.shape, np.int16)
-        lib.hc_quantize(len(d), q, _p(tabs), _p(d), _p(zz))
+        lib.hc_quantize(len(d), q, ptr(tabs), ptr(d), ptr(zz))
         qt = J.quant_tables(q)
         want = np.where(tabs[:, None] == 0, J.quantize(d, qt[0]), J.quantize(d, qt[1]))[:, J.ZIGZAG]
         assert np.array_equal(zz, want), q
@@ -186,20 +168,20 @@ def test_bits_packing_and_stuffing(lib):
     want_dc = np.where(tabs == 0, J.DC_CODES[0][1][s], J.DC_CODES[1][1][s]) + s
     want_all = np.bincount(blk, weights=lens, minlength=n).astype(np.int64)
     dc, ac = np.zeros(n, np.int32), np.zeros(n, np.int32)
-    lib.hc_block_bits(n, _p(zz), _p(diffs), _p(tabs), _p(dc), _p(ac))
+    lib.hc_block_bits(n, ptr(zz), ptr(diffs), ptr(tabs), ptr(dc), ptr(ac))
     assert np.array_equal(dc, want_dc) and np.array_equal(dc + ac, want_all)
     assert 1600 < (dc + ac).max() <= 1660                            # JPEG_BLOCK_MAX_BITS bounds the longest block
     offs = np.ascontiguousarray(np.cumsum(want_all) - want_all, np.uint64)
     total = int(want_all.sum())
     words = np.zeros(total // 32 + 2, np.uint32)
-    lib.hc_pack(n, _p(zz), _p(diffs), _p(tabs), _p(offs), total, _p(words))
+    lib.hc_pack(n, ptr(zz), ptr(diffs), ptr(tabs), ptr(offs), total, ptr(words))
     want = J.pack(vals, lens)
     got = words.byteswap().view(np.uint8)[:len(want)]
     assert np.array_equal(got, want)
     assert (want == 0xFF).sum() > 100                                # the stream holds many bytes to stuff
     for chunk in (1, 3, 16, 4096):
         out = np.zeros(2 * len(want) + 16, np.uint8)
-        m = lib.hc_stuff(_p(words), len(want), chunk, _p(out))
+        m = lib.hc_stuff(ptr(words), len(want), chunk, ptr(out))
         assert np.array_equal(out[:m], J.stuff(want)), chunk
 
 
@@ -210,7 +192,7 @@ def test_stuffing_of_a_stream_of_ones(lib):
     words = np.frombuffer(np.concatenate([data, np.zeros(4, np.uint8)]).tobytes(), np.uint32).byteswap().copy()
     for chunk in (1, 2, 7, 16):
         out = np.zeros(256, np.uint8)
-        m = lib.hc_stuff(_p(words), 100, chunk, _p(out))
+        m = lib.hc_stuff(ptr(words), 100, chunk, ptr(out))
         assert np.array_equal(out[:m], J.stuff(data)), chunk
 
 
@@ -222,10 +204,10 @@ def test_host_build_equals_cv2(lib, h, w):
             img = J.make_image(content, h, w, seed=3)
             cap = lib.hc_bound(w, h)
             out = np.zeros(cap, np.uint8)
-            n = lib.hc_encode(_p(img), 1, w, h, q, _p(out), cap)
+            n = lib.hc_encode(ptr(img), 1, w, h, q, ptr(out), cap)
             want = J.cv2_encode(img, q)
             assert n == len(want) and np.array_equal(out[:n], want), (content, q)
-            assert lib.hc_encode(_p(img), 1, w, h, q, _p(out), len(want) - 1) == -1
+            assert lib.hc_encode(ptr(img), 1, w, h, q, ptr(out), len(want) - 1) == -1
 
 
 def test_host_build_tiles_equal_hstack(lib):
@@ -233,7 +215,7 @@ def test_host_build_tiles_equal_hstack(lib):
         frames = np.stack([J.make_image("dots", th, tw, seed=s) for s in range(tiles)])
         cap = lib.hc_bound(tiles * tw, th)
         out = np.zeros(cap, np.uint8)
-        n = lib.hc_encode(_p(frames), tiles, tw, th, 95, _p(out), cap)
+        n = lib.hc_encode(ptr(frames), tiles, tw, th, 95, ptr(out), cap)
         assert np.array_equal(out[:n], J.cv2_encode(np.hstack(list(frames)), 95)), tiles
 
 

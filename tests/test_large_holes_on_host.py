@@ -4,7 +4,6 @@ full-size reduction of csrc/blob_device.cuh through tests/hostcheck/simt_emu.h w
 order, A2 / SX6 / SY6 of every contour, the pixel count of every hole region -- on holed blobs wider or taller than
 62 px: rings and frames up to the whole image, shapes across the border, a spiral, 16 and 40 nested frames, blobs and
 holed blobs inside large holes, 64-hole bands, and both windows in one image."""
-import ctypes
 import os
 import shutil
 import subprocess
@@ -12,30 +11,26 @@ import subprocess
 import numpy as np
 import pytest
 
+from tests import hostbuild
+from tests.hostbuild import HC, ROOT, ptr
 from tests.large_holes_util import large_holes_fuzz, nested_frames, spiral, wide_porous
-from tests.util import ROOT, retr_tree_blobs, set_pixel_blobs
+from tests.util import retr_tree_blobs, set_pixel_blobs
 
 pytestmark = pytest.mark.timeout(600)
 
-HC = os.path.join(ROOT, "tests", "hostcheck")
-CUDA_INC = os.path.join(os.environ.get("CUDA_HOME", "/usr/local/cuda"), "include")
 F_BLOBS, F_HOLES = 2, 32
 
 
 @pytest.fixture(scope="module")
-def large_emu(tmp_path_factory):
-    out = str(tmp_path_factory.mktemp("hc") / "libblob_large_holes.so")
-    subprocess.check_call(["g++", "-std=c++20", "-O2", "-shared", "-fPIC", "-pthread", "-I" + CUDA_INC, "-Wno-attributes",
-                           "-fno-strict-aliasing", "-o", out, os.path.join(HC, "blob_large_holes_host.cpp")])
-    lib = ctypes.CDLL(out)
+def large_emu():
+    lib = hostbuild.load("blob_large_holes")
 
     def detect(img, large=1, max_blobs=64, E=4096, seed=1):
         img = np.ascontiguousarray(img, dtype=np.uint8)
         H, W = img.shape
         xy = np.zeros((max_blobs, 2), np.int32); n = np.zeros(1, np.int32)
         mom = np.zeros((max_blobs, 4), np.int64); fl = np.zeros(1, np.int32)
-        p = lambda a: a.ctypes.data_as(ctypes.c_void_p)
-        rc = lib.hc_blob_detect_large(p(img), W, H, 51, max_blobs, E, large, seed, p(xy), p(n), p(mom), p(fl))
+        rc = lib.hc_blob_detect_large(ptr(img), W, H, 51, max_blobs, E, large, seed, ptr(xy), ptr(n), ptr(mom), ptr(fl))
         assert rc >= 0, rc
         k = int(n[0])
         return [tuple(int(v) for v in mom[i]) + tuple(int(v) for v in xy[i]) for i in range(k)], int(fl[0])
@@ -136,13 +131,8 @@ def test_whole_image_window_has_no_data_races(tmp_path):
     hole, a 65-hole band): the band flood, the CTA-wide minimum and sums and the hole records are race-free.  The
     union-find races by design and is suppressed, as in test_device_code_on_host.py; so would the 64 x 64 window's
     one-warp flood (it reads rows other lanes are growing), which is why no holed blob here fits that window."""
-    tsan = subprocess.run(["gcc", "-print-file-name=libtsan.so"], capture_output=True, text=True).stdout.strip()
-    if not tsan or not os.path.isabs(tsan) or not os.path.exists(tsan):
-        pytest.skip("libtsan not available")
-    lib = str(tmp_path / "liblarge_tsan.so")
-    subprocess.check_call(["g++", "-std=c++20", "-O1", "-g", "-fsanitize=thread", "-shared", "-fPIC", "-pthread", "-I" + CUDA_INC,
-                           "-Wno-attributes", "-Wno-tsan", "-fno-strict-aliasing", "-o", lib,
-                           os.path.join(HC, "blob_large_holes_host.cpp")])
+    env = hostbuild.tsan_env(tmp_path, ["race:uf_find", "race:uf_unite", "race:atomicMin"])
+    lib = hostbuild.build("blob_large_holes", tsan=True)
     import cv2
     imgs = []
     img = np.zeros((64, 96), np.uint8); spiral(img, 1, 1, 94, 62); imgs.append(img)
@@ -158,10 +148,7 @@ def test_whole_image_window_has_no_data_races(tmp_path):
         want, flags = (set_pixel_blobs(img > 0), F_HOLES) if k == 3 else (retr_tree_blobs(img > 0)[0], 0)
         cases.update({f"img{k}": img, f"want{k}": np.array(want, np.int64).reshape(-1, 6), f"flags{k}": flags})
     np.savez(tmp_path / "cases.npz", **cases)
-    supp = tmp_path / "supp.txt"
-    supp.write_text("race:uf_find\nrace:uf_unite\nrace:atomicMin\n")
-    env = dict(os.environ, LD_PRELOAD=tsan, TSAN_OPTIONS=f"report_signal_unsafe=0 history_size=4 exitcode=0 suppressions={supp}")
-    r = subprocess.run([shutil.which("python") or "python", os.path.join(HC, "tsan_large_holes_run.py"), lib, str(tmp_path / "cases.npz")],
+    r = subprocess.run([shutil.which("python") or "python", os.path.join(HC, "tsan_large_holes_run.py"), ROOT, lib, str(tmp_path / "cases.npz")],
                        capture_output=True, text=True, env=env, timeout=560)
     out = r.stdout + r.stderr
     assert out.count("LARGE True") == 4, out[-2000:]

@@ -1,16 +1,15 @@
 """The live loop's CPU tier: the host build of csrc/live.cuh (k_live_blobs's step code) against numpy on random blob
 lists; the host part of the drop-in _camera_read (api.live_read_events), fed the oracle chain's outputs, against the
 real reference's events and serial bytes in tests/golden/live_loop.npz; install_into(live=True)."""
-import ctypes
 import importlib
 import json
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
-from tests.live_util import (CAPTURE, DIST, K, LOCATE, ROOT, TRIANGULATE, encode_events, golden_scene, load_golden,
+from tests import hostbuild
+from tests.hostbuild import ptr
+from tests.live_util import (CAPTURE, DIST, K, LOCATE, TRIANGULATE, encode_events, golden_scene, load_golden,
                              oracle_read, render_read)
 
 api = importlib.import_module("low-cost-mocap_b200.api")
@@ -18,19 +17,8 @@ pkg = importlib.import_module("low-cost-mocap_b200")
 
 
 @pytest.fixture(scope="module")
-def lib(tmp_path_factory):
-    out = os.path.join(str(tmp_path_factory.mktemp("live")), "liblive_host.so")
-    subprocess.check_call(["g++", "-O2", "-shared", "-fPIC", "-ffp-contract=off", "-std=c++17", "-o", out,
-                           os.path.join(ROOT, "tests", "hostcheck", "live_host.cpp")])
-    lib = ctypes.CDLL(out)
-    P, I = ctypes.c_void_p, ctypes.c_int
-    lib.hc_live.restype = None
-    lib.hc_live.argtypes = [P, P, P, I, I, I, I, I, I, P, P, P, P, P, P]
-    return lib
-
-
-def _p(a):
-    return a.ctypes.data_as(ctypes.c_void_p) if a is not None else None
+def lib():
+    return hostbuild.load("live")
 
 
 @pytest.mark.parametrize("C,MB,mode,have", [(4, 64, CAPTURE, 1), (2, 8, CAPTURE | TRIANGULATE, 1),
@@ -50,8 +38,8 @@ def test_host_build_equals_numpy(lib, C, MB, mode, have):
                called=np.full(n, 9, np.uint8), flags=set_fl.copy())
     frames = rng.integers(0, 256, (n, C, S, S, 3), dtype=np.uint8)
     before = frames.copy()
-    lib.hc_live(_p(xy), _p(cnt), _p(fl), n, C, MB, S, have, mode, _p(out["cnt"]), _p(out["first"]), _p(out["gate"]), _p(out["called"]),
-                _p(out["flags"]), _p(frames))
+    lib.hc_live(ptr(xy), ptr(cnt), ptr(fl), n, C, MB, S, have, mode, ptr(out["cnt"]), ptr(out["first"]), ptr(out["gate"]), ptr(out["called"]),
+                ptr(out["flags"]), ptr(frames))
     eff = cnt if have else np.zeros_like(cnt)
     assert np.array_equal(out["cnt"], eff)
     want_first = np.where(eff[:, :, None] > 0, xy[:, :, 0, :], -1)

@@ -7,14 +7,15 @@ import hashlib
 import numpy as np
 import pytest
 
-from tests.locate_util import (D1, D2, GOLDEN, HEADING_TOL, MAX_POINTS, TOL, build_locate_host, compare_to_oracle, count_cases,
+from tests import hostbuild
+from tests.locate_util import (D1, D2, GOLDEN, HEADING_TOL, MAX_POINTS, TOL, compare_to_oracle, count_cases,
                                edge_scenes, equal_but_heading, fold_allowed, fuzz_scenes, golden_fuzz_scenes, host_locate,
                                host_locate_batch, large_scenes, oracle, pack, small_scenes, trace)
 
 
 @pytest.fixture(scope="module")
-def lib(tmp_path_factory):
-    return build_locate_host(tmp_path_factory.mktemp("locate"))
+def lib():
+    return hostbuild.load("locate")
 
 
 # ---------------------------------------------------------------------------------------------- the oracle

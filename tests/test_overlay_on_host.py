@@ -1,41 +1,20 @@
 """The detection overlay's CPU tier: the host build of csrc/overlay.cuh (the drawing code of the overlay kernels) against
 cv2 -- the contour stencil, the plus marks, the '(x, y)' labels, the line rasteriser -- and the whole of _find_dot's
 drawing on random frames and on the live session's frames."""
-import ctypes
-import os
-import subprocess
-
 import cv2
 import numpy as np
 import pytest
 
+from tests import hostbuild
+from tests.hostbuild import ptr
 from tests.overlay_util import drawline_of, find_dot_drawn, random_scene
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 MARK = (100, 255, 100)
 
 
 @pytest.fixture(scope="module")
-def lib(tmp_path_factory):
-    out = os.path.join(str(tmp_path_factory.mktemp("overlay")), "liboverlay_host.so")
-    subprocess.check_call(["g++", "-O2", "-shared", "-fPIC", "-ffp-contract=off", "-std=c++17", "-o", out,
-                           os.path.join(ROOT, "tests", "hostcheck", "overlay_host.cpp")])
-    lib = ctypes.CDLL(out)
-    P, I, L = ctypes.c_void_p, ctypes.c_int, ctypes.c_int64
-    lib.hc_overlay.restype = lib.hc_label.restype = lib.hc_plus.restype = lib.hc_line.restype = None
-    lib.hc_overlay.argtypes = [P, I, I, I, I, P, P]
-    lib.hc_label.argtypes = lib.hc_plus.argtypes = [P, I, I, I, I]
-    lib.hc_line.argtypes = [P, I, I, L, L, L, L, I]
-    lib.hc_line_lanes.restype = lib.hc_palette.restype = None
-    lib.hc_line_lanes.argtypes = [P, I, I, L, L, L, L, I]
-    lib.hc_palette.argtypes = [ctypes.c_uint32, I, P]
-    lib.hc_epiline_ends.restype = I
-    lib.hc_epiline_ends.argtypes = [ctypes.c_float, ctypes.c_float, ctypes.c_float, I, P, P]
-    return lib
-
-
-def _p(a):
-    return a.ctypes.data_as(ctypes.c_void_p) if a is not None else None
+def lib():
+    return hostbuild.load("overlay")
 
 
 def _overlay(lib, img, pts):
@@ -43,7 +22,7 @@ def _overlay(lib, img, pts):
     out = np.ascontiguousarray(img.copy())
     H, W = img.shape[:2]
     xy = np.array(pts if pts else [[0, 0]], np.int32).reshape(1, -1, 2)
-    lib.hc_overlay(_p(out), 1, W, H, xy.shape[1], _p(xy), _p(np.array([len(pts)], np.int32)))
+    lib.hc_overlay(ptr(out), 1, W, H, xy.shape[1], ptr(xy), ptr(np.array([len(pts)], np.int32)))
     return out
 
 
@@ -87,7 +66,7 @@ def test_plus_at_every_position(lib):
             want = np.zeros((7, 9, 3), np.uint8)
             cv2.circle(want, (x, y), 1, MARK, -1)
             got = np.zeros_like(want)
-            lib.hc_plus(_p(got), 9, 7, x, y)
+            lib.hc_plus(ptr(got), 9, 7, x, y)
             assert np.array_equal(got, want), (x, y)
 
 
@@ -105,7 +84,7 @@ def test_labels_of_every_coordinate_pair_up_to_1023(lib):
         want = np.zeros((S, S, 3), np.uint8)
         cv2.putText(want, f'({x}, {y})', (x, y - 15), cv2.FONT_HERSHEY_SIMPLEX, 0.3, MARK, 1)
         frame[:] = 0
-        lib.hc_label(_p(frame), S, S, x, y)
+        lib.hc_label(ptr(frame), S, S, x, y)
         y0, y1, x0, x1 = max(0, y - 30), min(S, y + 10), max(0, x - 5), min(S, x + 80)
         assert np.array_equal(frame[y0:y1, x0:x1], want[y0:y1, x0:x1]) and frame.sum() == want.sum(), (x, y)
     # small frames: the labels of centres near every edge clip at the frame's sides; centres off the frame, negative
@@ -116,7 +95,7 @@ def test_labels_of_every_coordinate_pair_up_to_1023(lib):
                 want = np.zeros((H, W, 3), np.uint8)
                 cv2.putText(want, f'({x}, {y})', (x, y - 15), cv2.FONT_HERSHEY_SIMPLEX, 0.3, MARK, 1)
                 got = np.zeros_like(want)
-                lib.hc_label(_p(got), W, H, x, y)
+                lib.hc_label(ptr(got), W, H, x, y)
                 assert np.array_equal(got, want), (W, H, x, y)
 
 
@@ -139,13 +118,13 @@ def test_lines_equal_cv2(lib):
         want = np.zeros((H, W, 3), np.uint8)
         cv2.line(want, (int(p[0]), int(p[1])), (int(p[2]), int(p[3])), MARK, 1, cv2.LINE_8)
         got = np.zeros_like(want)
-        lib.hc_line(_p(got), W, H, *[int(v) for v in p], 0)
+        lib.hc_line(ptr(got), W, H, *[int(v) for v in p], 0)
         assert np.array_equal(got, want), p
         q = rng.integers(-8 << 16, 56 << 16, 4)
         want = np.zeros((H, W, 3), np.uint8)
         cv2.line(want, (int(q[0]), int(q[1])), (int(q[2]), int(q[3])), MARK, 1, cv2.LINE_8, 16)
         got = np.zeros_like(want)
-        lib.hc_line(_p(got), W, H, *[int(v) for v in q], 1)
+        lib.hc_line(ptr(got), W, H, *[int(v) for v in q], 1)
         assert np.array_equal(got, want), q
 
 
@@ -172,7 +151,7 @@ def test_palette_is_numpys_legacy_randint(lib):
     after np.random.seed(seed), as the reference draws its line colours."""
     for seed in (0, 11, 2 ** 32 - 1):
         got = np.zeros((5000, 3), np.uint8)
-        lib.hc_palette(seed, 5000, _p(got))
+        lib.hc_palette(seed, 5000, ptr(got))
         assert np.array_equal(got, np.random.RandomState(seed).randint(0, 255, (5000, 3)))
         state = np.random.get_state()
         try:
@@ -197,7 +176,7 @@ def test_epipolar_line_end_points_and_skips(lib):
         c = rng.uniform(-1, 1) * 10.0 ** rng.integers(0, 8) if t % 7 else 0.0
         r = np.array([a, b, c], np.float32)
         y0, y1 = np.zeros(1, np.int64), np.zeros(1, np.int64)
-        ok = lib.hc_epiline_ends(float(r[0]), float(r[1]), float(r[2]), W, _p(y0), _p(y1))
+        ok = lib.hc_epiline_ends(float(r[0]), float(r[1]), float(r[2]), W, ptr(y0), ptr(y1))
         want = np.zeros((H, W, 3), np.uint8)
         ref_ok = drawline_of(want, r, (3, 200, 17))
         assert bool(ok) == ref_ok, r
@@ -209,6 +188,6 @@ def test_epipolar_line_end_points_and_skips(lib):
             assert (y0[0], y1[0]) == (int(-r[2] / r[1]), int(-(r[2] + r[0] * W) / r[1])), r
         for lanes in (1, 32):
             got = np.zeros_like(want)
-            lib.hc_line_lanes(_p(got), W, H, 0, int(y0[0]), W, int(y1[0]), lanes)
+            lib.hc_line_lanes(ptr(got), W, H, 0, int(y0[0]), W, int(y1[0]), lanes)
             assert np.array_equal(got.any(2), want.any(2)), (r, lanes)
     assert skipped > 100 and drawn > 2000

@@ -7,6 +7,7 @@ import os
 import numpy as np
 import pytest
 
+from tests.hostbuild import ptr
 from tests.util import load_golden, poses_from, obs_from, as3
 
 pytestmark = pytest.mark.gpu
@@ -426,8 +427,7 @@ def test_ba_reference_iteration_only(torch):
     rep = _l.BAReport()
     R = np.ascontiguousarray(z["R_start"].copy()); t = np.ascontiguousarray(z["t_start"].copy())
     obs = np.ascontiguousarray(z["obs"]); mask = np.ascontiguousarray(z["mask"])
-    p = lambda a: a.ctypes.data_as(Ct.c_void_p)
-    st = lib.mocap_bundle_adjust_host(ctx.h, p(obs), p(mask), obs.shape[0], p(R), p(t), Ct.byref(opt), Ct.byref(rep))
+    st = lib.mocap_bundle_adjust_host(ctx.h, ptr(obs), ptr(mask), obs.shape[0], ptr(R), ptr(t), Ct.byref(opt), Ct.byref(rep))
     assert st == 0
     assert abs(rep.cost_initial - float(z["cost0"])) < 1e-3 * float(z["cost0"])
     assert rep.cost_final < rep.cost_initial and rep.status in (0, 1, 2, 3, 4)

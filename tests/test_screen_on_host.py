@@ -8,7 +8,8 @@ import numpy as np
 import pytest
 
 from oracle.ref_port import RefPort
-from tests.screen_util import build_screen_host, contaminated_tracks, host_screen, screen_inputs
+from tests import hostbuild
+from tests.screen_util import contaminated_tracks, host_screen, screen_inputs
 
 synth = importlib.import_module("low-cost-mocap_b200.synth")
 THR = 4.0
@@ -16,8 +17,8 @@ NEAR = 1e-6          # px: rows with a compared error this close to the threshol
 
 
 @pytest.fixture(scope="module")
-def lib(tmp_path_factory):
-    return build_screen_host(tmp_path_factory.mktemp("screen"))
+def lib():
+    return hostbuild.load("screen")
 
 
 def restate_row(port, o, m, poses, thr):

@@ -2,14 +2,15 @@
 oracle equals the real reference's KalmanFilter on tests/golden/track_live.npz bit for bit, the low-pass filter equals
 scipy's lfilter bit for bit, and the host build follows the oracle on the golden stream and on seeded synthetic ones
 (association and heading exact, pos / vel within a float32 tolerance).  Also install_into(tracker=...)."""
-import ctypes
 import importlib
 
 import numpy as np
 import pytest
 from scipy.signal import butter, lfilter
 
-from tests.track_util import build_track_host, golden_stream, host_run, load_golden, make_stream, run_oracle
+from tests import hostbuild
+from tests.hostbuild import ptr
+from tests.track_util import golden_stream, host_run, load_golden, make_stream, run_oracle
 
 TOL = 5e-5                # pos / vel against the oracle; cv2 solves the gain by a float32 SVD, the step code in double
 TOL_AFTER_RESET = 5e-4    # the calls after reset(): see test_host_build_follows_the_oracle_on_the_golden_stream
@@ -17,8 +18,8 @@ SPLITS = (1, 7, 299, 301)
 
 
 @pytest.fixture(scope="module")
-def lib(tmp_path_factory):
-    return build_track_host(tmp_path_factory.mktemp("track"))
+def lib():
+    return hostbuild.load("track")
 
 
 @pytest.fixture(scope="module")
@@ -37,7 +38,7 @@ def test_oracle_equals_the_reference_on_the_golden_stream(golden):
 
 def test_lowpass_coefficients_are_butter(lib):
     b, a = np.zeros(6), np.zeros(6)
-    lib.hc_lowpass_coefs(b.ctypes.data_as(ctypes.c_void_p), a.ctypes.data_as(ctypes.c_void_p))
+    lib.hc_lowpass_coefs(ptr(b), ptr(a))
     bb, aa = butter(5, 20 / 30)
     assert np.array_equal(b, bb) and np.array_equal(a, aa)
 
@@ -49,7 +50,7 @@ def test_lowpass_equals_lfilter_for_every_window(lib):
     for scale in (1.0, 3e-3, 40.0):
         x = np.ascontiguousarray(rng.normal(0, scale, 300))
         for L in range(1, 301):
-            got = lib.hc_lowpass(x[300 - L:].ctypes.data_as(ctypes.c_void_p), L)
+            got = lib.hc_lowpass(ptr(x[300 - L:]), L)
             assert got == lfilter(b, a, x[300 - L:])[-1], (scale, L)
 
 

@@ -1,14 +1,14 @@
 """Helpers shared by the CPU and GPU tests of the drone tracker (csrc/track.cuh, csrc/track.cu), the golden generator
 tests/golden/make_golden_track.py and tools/track_time.py: seeded streams of located frame-sets in the layout
 mocap_locate_objects_dev writes, a restatement of the reference's KalmanFilter / LowPassFilter with an injectable clock
-(the oracle of the tracker), and the g++ build of the step code."""
-import ctypes
+(the oracle of the tracker), and the host build of the step code behind api.Tracker's interface."""
 import os
-import subprocess
 
 import cv2
 import numpy as np
 from scipy.signal import butter, lfilter
+
+from tests.hostbuild import ptr
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden", "track_live.npz")
@@ -198,25 +198,6 @@ def run_oracle(stream, D):
 
 
 # ---------------------------------------------------------------------------------------------- host build
-def build_track_host(tmpdir):
-    """g++ build of csrc/track.cuh (tests/hostcheck/track_host.cpp) -> ctypes library."""
-    out = os.path.join(str(tmpdir), "libtrack_host.so")
-    subprocess.check_call(["g++", "-O2", "-shared", "-fPIC", "-ffp-contract=off", "-std=c++17", "-o", out,
-                           os.path.join(ROOT, "tests", "hostcheck", "track_host.cpp"), "-lm"])
-    lib = ctypes.CDLL(out)
-    P, I, Dbl = ctypes.c_void_p, ctypes.c_int, ctypes.c_double
-    for name, res, args in (("hc_track_new", P, [I]), ("hc_track_free", None, [P]), ("hc_track_reset", None, [P, Dbl]),
-                            ("hc_track", None, [P, P, P, P, I, P, I, P, P, P, P, P]), ("hc_lowpass", Dbl, [P, I]),
-                            ("hc_window", I, [I]), ("hc_next_call", I, [I]), ("hc_lowpass_coefs", None, [P, P])):
-        fn = getattr(lib, name)
-        fn.restype, fn.argtypes = res, args
-    return lib
-
-
-def _p(a):
-    return a.ctypes.data_as(ctypes.c_void_p)
-
-
 class HostTracker:
     """The host build with the interface of api.Tracker, on numpy arrays."""
 
@@ -236,8 +217,8 @@ class HostTracker:
         B, M = drone_index.shape
         out = dict(pos=np.zeros((B, self.D, 3), np.float32), vel=np.zeros((B, self.D, 3), np.float32),
                    heading=np.zeros((B, self.D)), present=np.zeros((B, self.D), np.uint8), chosen=np.zeros((B, self.D), np.int32))
-        self.lib.hc_track(self.h, _p(objects), _p(drone_index), _p(n), M, _p(t), B, _p(out["pos"]), _p(out["vel"]),
-                          _p(out["heading"]), _p(out["present"]), _p(out["chosen"]))
+        self.lib.hc_track(self.h, ptr(objects), ptr(drone_index), ptr(n), M, ptr(t), B, ptr(out["pos"]), ptr(out["vel"]),
+                          ptr(out["heading"]), ptr(out["present"]), ptr(out["chosen"]))
         return out
 
 
