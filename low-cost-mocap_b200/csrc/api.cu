@@ -49,6 +49,44 @@ static int ensure_sets(mocap_ctx* ctx, int n_sets) {
     return st;
 }
 
+// Single-pass kernel or three-kernel pipeline for this batch of 1-channel frames?  The single-pass kernel wins
+// while the sparse stages are light (config 2: 4.34 ms against 4.70 ms per 10 000 frame-sets on an H100 SXM at a
+// 400 W power limit); with many blobs per frame-set the sparse stages interleaved with the stream loop on every SM
+// hold back the stream (config 3 shape: 5.68 ms against 5.29 ms per 4000 frame-sets), so batches that follow a heavy
+// batch take the three-kernel pipeline.  The blob count of the previous batch arrives through mapped host memory
+// (written by the last CTA of the blob fallback kernel): no synchronisation, a stale or torn value only steers
+// this heuristic, both pipelines give the same results.
+bool pick_fused(const mocap_ctx* ctx) {
+    if (!ctx->use_fused) return false;
+    if (!ctx->pipeline_auto) return true;
+    const volatile unsigned long long* h_stat = ctx->stat_host.as<volatile unsigned long long>();
+    const unsigned long long blobs = h_stat[0], images = h_stat[1];
+    if (images == 0) return true;
+    return (double)blobs * ctx->cfg.n_cam <= (double)MOCAP_HEAVY_BLOBS_PER_SET * (double)images;
+}
+
+// Launch groups bound the detection scratch (max_segments * 4 B of segment list per image) at any batch size: 65 536
+// images for the single-pass kernel, 4096 frame-sets for the three-kernel pipeline.
+int run_sets(mocap_ctx* ctx, const uint8_t* frames, int n_sets, int channels, int threshold, bool fused, const SetOut& out,
+             cudaEvent_t frames_read) {
+    const int C = ctx->cfg.n_cam;
+    const size_t set_bytes = (size_t)C * ctx->cfg.width * ctx->cfg.height * channels;
+    const int group = fused ? (65536 / C > 0 ? 65536 / C : 1) : 4096;
+    int st = ensure_images(ctx, (n_sets < group ? n_sets : group) * C);
+    if (st) return st;
+    for (int s0 = 0; s0 < n_sets; s0 += group) {
+        const int ns = (n_sets - s0 < group) ? n_sets - s0 : group;
+        const uint8_t* f = frames + (size_t)s0 * set_bytes;
+        const SetOut o = out.at(ctx->cfg, s0);      // frame-set indices inside a launch group start at 0
+        st = fused ? launch_pipeline_fused(ctx, f, ns, channels, threshold, o)
+                   : launch_detect(ctx, f, ns * C, channels, threshold, ctx->d_blob_xy, ctx->d_blob_n, nullptr, ctx->d_img_flags);
+        if (st) return st;
+        if (frames_read) CUDA_TRY(ctx, cudaEventRecord(frames_read, ctx->stream));
+        if (!fused && (st = launch_match(ctx, ctx->d_blob_xy, ctx->d_blob_n, ns, o, ctx->d_img_flags, nullptr)) != MOCAP_OK) return st;
+    }
+    return MOCAP_OK;
+}
+
 extern "C" {
 
 const char* mocap_status_string(int status) {
@@ -188,22 +226,6 @@ int mocap_set_world_transform(mocap_ctx* ctx, const double* M) {
     return MOCAP_OK;
 }
 
-// Single-pass kernel or three-kernel pipeline for this batch of 1-channel frames?  The single-pass kernel wins
-// while the sparse stages are light (config 2: 4.34 ms against 4.70 ms per 10 000 frame-sets on an H100 SXM at a
-// 400 W power limit); with many blobs per frame-set the sparse stages interleaved with the stream loop on every SM
-// hold back the stream (config 3 shape: 5.68 ms against 5.29 ms per 4000 frame-sets), so batches that follow a heavy
-// batch take the three-kernel pipeline.  The blob count of the previous batch arrives through mapped host memory
-// (written by the last CTA of the blob fallback kernel): no synchronisation, a stale or torn value only steers
-// this heuristic, both pipelines give the same results.
-static bool pick_fused(const mocap_ctx* ctx) {
-    if (!ctx->use_fused) return false;
-    if (!ctx->pipeline_auto) return true;
-    const volatile unsigned long long* h_stat = ctx->stat_host.as<volatile unsigned long long>();
-    const unsigned long long blobs = h_stat[0], images = h_stat[1];
-    if (images == 0) return true;
-    return (double)blobs * ctx->cfg.n_cam <= (double)MOCAP_HEAVY_BLOBS_PER_SET * (double)images;
-}
-
 // ---- S1 ------------------------------------------------------------------------------------
 int mocap_detect_dev(mocap_ctx* ctx, const uint8_t* frames, int n_images, int channels, int threshold,
                      int32_t* blob_xy, int32_t* blob_n, int64_t* blob_mom, int32_t* img_flags) {
@@ -226,7 +248,7 @@ int mocap_match_triangulate_dev(mocap_ctx* ctx, const int32_t* blob_xy, const in
         return mocap_fail(ctx, MOCAP_EINVAL, "mocap_match_triangulate_dev: bad argument");
     if (!ctx->cameras_set) return mocap_fail(ctx, MOCAP_ESTATE, "mocap_set_cameras has not been called");
     CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));
-    return launch_match(ctx, blob_xy, blob_n, n_frame_sets, obj, err, n_obj, set_flags, chosen);
+    return launch_match(ctx, blob_xy, blob_n, n_frame_sets, SetOut{obj, err, n_obj, set_flags, nullptr}, nullptr, chosen);
 }
 
 // ---- S1+S2+S3 ------------------------------------------------------------------------------
@@ -242,34 +264,7 @@ int mocap_pipeline_tracks_dev(mocap_ctx* ctx, const uint8_t* frames, int n_frame
         return mocap_fail(ctx, MOCAP_EINVAL, "mocap_pipeline_dev: bad argument");
     if (!ctx->cameras_set) return mocap_fail(ctx, MOCAP_ESTATE, "mocap_set_cameras has not been called");
     CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));
-    const int C = ctx->cfg.n_cam;
-    const size_t set_bytes = (size_t)C * ctx->cfg.width * ctx->cfg.height * channels;
-    const bool fused = pick_fused(ctx);
-    // frame-sets per launch group: bounds the segment-list scratch (max_segments * 4 B per image)
-    const int chunk = fused ? (65536 / C > 0 ? 65536 / C : 1) : 4096;
-    int st = ensure_images(ctx, (n_frame_sets < chunk ? n_frame_sets : chunk) * C);
-    if (st) return st;
-    for (int s0 = 0; s0 < n_frame_sets; s0 += chunk) {
-        const int ns = (n_frame_sets - s0 < chunk) ? n_frame_sets - s0 : chunk;
-        // the launchers hand this to the matcher (frame-set indices inside a launch group start at 0)
-        ctx->track_xy_cur = track_xy ? track_xy + (size_t)s0 * ctx->cfg.max_roots * C * 2 : nullptr;
-        if (fused) {
-            st = launch_pipeline_fused(ctx, frames + (size_t)s0 * set_bytes, ns, threshold, obj + (size_t)s0 * ctx->cfg.max_roots * 3,
-                                       err + (size_t)s0 * ctx->cfg.max_roots, n_obj + s0, set_flags ? set_flags + s0 : nullptr, channels);
-            if (st) break;
-            continue;
-        }
-        st = launch_detect(ctx, frames + (size_t)s0 * set_bytes, ns * C, channels, threshold,
-                           ctx->d_blob_xy, ctx->d_blob_n, nullptr, ctx->d_img_flags);
-        if (st) break;
-        ctx->img_flags_cur = ctx->d_img_flags;
-        st = launch_match(ctx, ctx->d_blob_xy, ctx->d_blob_n, ns, obj + (size_t)s0 * ctx->cfg.max_roots * 3,
-                          err + (size_t)s0 * ctx->cfg.max_roots, n_obj + s0, set_flags ? set_flags + s0 : nullptr, nullptr);
-        ctx->img_flags_cur = nullptr;
-        if (st) break;
-    }
-    ctx->track_xy_cur = nullptr;
-    return st;
+    return run_sets(ctx, frames, n_frame_sets, channels, threshold, pick_fused(ctx), SetOut{obj, err, n_obj, set_flags, track_xy}, nullptr);
 }
 
 int mocap_pipeline_host(mocap_ctx* ctx, const uint8_t* frames, int n_frame_sets, int channels, int threshold,
@@ -291,14 +286,13 @@ int mocap_pipeline_host(mocap_ctx* ctx, const uint8_t* frames, int n_frame_sets,
     if (st) return st;
     st = ensure_sets(ctx, n_frame_sets);
     if (st) return st;
-    st = ensure_images(ctx, chunk * C);
-    if (st) return st;
     cudaEvent_t* copied = ctx->copied;
     // the copies must not start before earlier work on the caller's stream has finished with the staging buffers
     CUDA_TRY(ctx, cudaEventRecord(copied[0], ctx->stream));
     CUDA_TRY(ctx, cudaStreamWaitEvent(ctx->copy_stream, copied[0], 0));
     CUDA_TRY(ctx, cudaStreamWaitEvent(ctx->copy_stream2, copied[0], 0));
     const bool fused = pick_fused(ctx);
+    const SetOut out{ctx->d_obj, ctx->d_err, ctx->d_nobj, ctx->d_setflags, nullptr};
     int k = 0, n_chunks = 0;
     for (int s0 = 0; s0 < n_frame_sets; s0 += chunk, k ^= 1, ++n_chunks) {
         const int ns = (n_frame_sets - s0 < chunk) ? n_frame_sets - s0 : chunk;
@@ -308,23 +302,9 @@ int mocap_pipeline_host(mocap_ctx* ctx, const uint8_t* frames, int n_frame_sets,
                                       cudaMemcpyHostToDevice, cs));
         CUDA_TRY(ctx, cudaEventRecord(copied[k], cs));
         CUDA_TRY(ctx, cudaStreamWaitEvent(ctx->stream, copied[k], 0));
-        if (fused) {
-            st = launch_pipeline_fused(ctx, ctx->d_stage[k], ns, threshold, ctx->d_obj + (size_t)s0 * RM * 3, ctx->d_err + (size_t)s0 * RM,
-                                       ctx->d_nobj + s0, ctx->d_setflags + s0, channels);
-            if (st) break;
-            CUDA_TRY(ctx, cudaEventRecord(ctx->stage_free[k], ctx->stream));
-            continue;
-        }
-        st = launch_detect(ctx, ctx->d_stage[k], ns * C, channels, threshold, ctx->d_blob_xy, ctx->d_blob_n, nullptr, ctx->d_img_flags);
-        if (st) break;
-        CUDA_TRY(ctx, cudaEventRecord(ctx->stage_free[k], ctx->stream));
-        ctx->img_flags_cur = ctx->d_img_flags;
-        st = launch_match(ctx, ctx->d_blob_xy, ctx->d_blob_n, ns, ctx->d_obj + (size_t)s0 * RM * 3, ctx->d_err + (size_t)s0 * RM,
-                          ctx->d_nobj + s0, ctx->d_setflags + s0, nullptr);
-        ctx->img_flags_cur = nullptr;
-        if (st) break;
+        if ((st = run_sets(ctx, ctx->d_stage[k], ns, channels, threshold, fused, out.at(ctx->cfg, s0), ctx->stage_free[k])) != MOCAP_OK)
+            return st;
     }
-    if (st) return st;
     const size_t n = (size_t)n_frame_sets;
     CUDA_TRY(ctx, cudaMemcpyAsync(obj, ctx->d_obj, n * RM * 3 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
     CUDA_TRY(ctx, cudaMemcpyAsync(err, ctx->d_err, n * RM * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));

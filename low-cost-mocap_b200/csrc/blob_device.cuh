@@ -12,6 +12,14 @@
 // ---------------------------------------------------------------------------------------------
 struct ThreshConst { uint32_t addc; uint32_t use_and; };   // see swar_gt()
 
+// host: the constants of "pixel > threshold" (threshold < 0: every pixel passes; >= 255: none does)
+inline ThreshConst thresh_const(int threshold) {
+    if (threshold < 0) return {0x80808080u, 0u};
+    if (threshold >= 255) return {0u, 1u};
+    const uint32_t T1 = (uint32_t)threshold + 1u;
+    return {(T1 > 128 ? 256u - T1 : 128u - T1) * 0x01010101u, T1 > 128 ? 1u : 0u};
+}
+
 // bit 7 of every byte of the result is (byte > threshold).  T1 = threshold+1 in 1..255:
 //   T1 <= 128:  b >= T1  <=>  high bit set  OR  low7 + (128-T1) carries into bit 7
 //   T1 >  128:  b >= T1  <=>  high bit set  AND low7 + (256-T1) carries into bit 7

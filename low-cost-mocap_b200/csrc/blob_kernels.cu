@@ -212,19 +212,10 @@ int launch_detect(mocap_ctx* ctx, const uint8_t* frames, int n_images, int chann
     const int E = c.max_segments;
     if (n_images <= 0) return MOCAP_OK;
 
-    if (ctx->timing_on) {
-        if (ctx->tim_used == 64) { const int st = timing_flush(ctx); if (st) return st; }
-        CUDA_TRY(ctx, cudaEventRecord(ctx->tim_ev[2 * ctx->tim_used], ctx->stream));
-    }
+    int st = timing_begin(ctx);
+    if (st) return st;
     const int threads = 256;
-    ThreshConst tc;
-    if (threshold < 0) { tc.addc = 0x80808080u; tc.use_and = 0; }            // everything passes
-    else if (threshold >= 255) { tc.addc = 0; tc.use_and = 1; }              // nothing passes
-    else {
-        const uint32_t T1 = (uint32_t)threshold + 1u;
-        tc.use_and = T1 > 128 ? 1u : 0u;
-        tc.addc = (T1 > 128 ? 256u - T1 : 128u - T1) * 0x01010101u;
-    }
+    const ThreshConst tc = thresh_const(threshold);
     const long long cap = (long long)ctx->num_sms * 8;      // 8 CTAs of 256 threads fill an SM
     if (channels == 1) {
         constexpr int UNROLL = 8;
@@ -240,14 +231,9 @@ int launch_detect(mocap_ctx* ctx, const uint8_t* frames, int n_images, int chann
             reinterpret_cast<const uint4*>(frames), n_seg, seg_per_image, E, threshold, tc, ctx->d_seg_count, ctx->d_seg_list);
     }
     CUDA_TRY(ctx, cudaGetLastError());
-    if (ctx->timing_on) {
-        CUDA_TRY(ctx, cudaEventRecord(ctx->tim_ev[2 * ctx->tim_used + 1], ctx->stream));
-        ctx->tim_used += 1;
-    }
+    if ((st = timing_end(ctx)) != MOCAP_OK) return st;
     constexpr int WPB = 8;
-    const long long mx = c.width > c.height ? c.width : c.height;
-    const bool wide = 6ll * mx * c.width * c.height >= (1ll << 32);      // moment sums may exceed 32 bits
-    if (wide)
+    if (moments_wide(c))
         k_blob_reduce_warp<WPB, true><<<(n_images + WPB - 1) / WPB, WPB * 32, 0, ctx->stream>>>(
             ctx->d_seg_count, ctx->d_seg_list, n_images, E, c.width, c.height, c.max_blobs, blob_xy, blob_n, blob_mom, img_flags,
             ctx->d_worklist, ctx->d_work_count);
@@ -256,10 +242,7 @@ int launch_detect(mocap_ctx* ctx, const uint8_t* frames, int n_images, int chann
             ctx->d_seg_count, ctx->d_seg_list, n_images, E, c.width, c.height, c.max_blobs, blob_xy, blob_n, blob_mom, img_flags,
             ctx->d_worklist, ctx->d_work_count);
     CUDA_TRY(ctx, cudaGetLastError());
-    {
-        const int st = launch_blob_fallback(ctx, blob_xy, blob_n, blob_mom, img_flags, n_images);
-        if (st) return st;
-    }
+    if ((st = launch_blob_fallback(ctx, blob_xy, blob_n, blob_mom, img_flags, n_images)) != MOCAP_OK) return st;
     ctx->launches += 2;      // stream kernel + warp-level reduce (the fallback counted itself)
     return MOCAP_OK;
 }
@@ -271,9 +254,7 @@ int launch_blob_fallback(mocap_ctx* ctx, int32_t* blob_xy, int32_t* blob_n, int6
     const int E = c.max_segments;
     const size_t smem = blob_reduce_smem_bytes(E);
     const int grid2 = ctx->num_sms;
-    const long long mx = c.width > c.height ? c.width : c.height;
-    const bool wide = 6ll * mx * c.width * c.height >= (1ll << 32);
-    if (wide)
+    if (moments_wide(c))
         k_blob_reduce<NT, true><<<grid2, NT, smem, ctx->stream>>>(ctx->d_seg_count, ctx->d_seg_list, E, c.width, c.height,
                                                                c.max_blobs, blob_xy, blob_n, blob_mom, img_flags,
                                                                ctx->d_worklist, ctx->d_work_count, ctx->d_work_count + 1,
@@ -287,6 +268,20 @@ int launch_blob_fallback(mocap_ctx* ctx, int32_t* blob_xy, int32_t* blob_n, int6
                                                                ctx->hole_win.as<unsigned long long>());
     CUDA_TRY(ctx, cudaGetLastError());
     ctx->launches += 1;
+    return MOCAP_OK;
+}
+
+int timing_begin(mocap_ctx* ctx) {
+    if (!ctx->timing_on) return MOCAP_OK;
+    if (ctx->tim_used == 64) { const int st = timing_flush(ctx); if (st) return st; }
+    CUDA_TRY(ctx, cudaEventRecord(ctx->tim_ev[2 * ctx->tim_used], ctx->stream));
+    return MOCAP_OK;
+}
+
+int timing_end(mocap_ctx* ctx) {
+    if (!ctx->timing_on) return MOCAP_OK;
+    CUDA_TRY(ctx, cudaEventRecord(ctx->tim_ev[2 * ctx->tim_used + 1], ctx->stream));
+    ctx->tim_used += 1;
     return MOCAP_OK;
 }
 

@@ -80,8 +80,6 @@ struct mocap_ctx {
     DeviceBuffer match_split;
     unsigned* d_match_arrive; void* d_match_items; unsigned long long* d_match_partial; int* d_match_range;
     int match_chunk, match_item_cap, match_cap_sets;
-    const int32_t* img_flags_cur;   // set by the pipelines: the matcher folds the images' S1 flags into the frame-set's
-    int32_t*  track_xy_cur;   // set for the duration of mocap_pipeline_tracks_dev: where the matcher leaves the winners' pixels
     // capture-side preprocessing (SURVEY 8(f) #2); pp_in_w != 0 once mocap_set_preprocess has put all three maps on the device
     DeviceBuffer pp_m1, pp_m2, pp_rot; int pp_in_w, pp_in_h;
     // mocap_live_host staging: device and page-locked host buffers of {timestamps, raw frames} and {result, frames}
@@ -111,11 +109,22 @@ int mocap_fail(mocap_ctx* ctx, int code, const char* fmt, ...);
                               cudaGetErrorString(e__), __FILE__, __LINE__);              \
     } while (0)
 
+// What S2+S3 write per frame-set: obj [n][max_roots][3], err [n][max_roots], n [n], flags [n] (may be null) and the
+// winners' pixels track_xy [n][max_roots][n_cam][2] (may be null).  at(): the same record from frame-set s0 on.
+struct SetOut {
+    double* obj; double* err; int32_t* n; int32_t* flags; int32_t* track_xy;
+    SetOut at(const mocap_config& c, int s0) const {
+        const size_t s = (size_t)s0, R = (size_t)c.max_roots;
+        return {obj + s * R * 3, err + s * R, n + s, flags ? flags + s : nullptr, track_xy ? track_xy + s * R * c.n_cam * 2 : nullptr};
+    }
+};
+
 // kernel launchers (each returns a MOCAP_* status; all enqueue on ctx->stream)
 int launch_detect(mocap_ctx* ctx, const uint8_t* frames, int n_images, int channels, int threshold,
                   int32_t* blob_xy, int32_t* blob_n, int64_t* blob_mom, int32_t* img_flags);
-int launch_match(mocap_ctx* ctx, const int32_t* blob_xy, const int32_t* blob_n, int n_sets,
-                 double* obj, double* err, int32_t* n_obj, int32_t* set_flags, int32_t* chosen);
+// img_flags (may be null): the images' S1 flags, folded into each frame-set's flags; chosen (may be null)
+int launch_match(mocap_ctx* ctx, const int32_t* blob_xy, const int32_t* blob_n, int n_sets, const SetOut& out,
+                 const int32_t* img_flags, int32_t* chosen);
 int launch_triangulate(mocap_ctx* ctx, const double* obs, const uint8_t* mask, int n_points,
                        const double* X_in, double* X, double* err, uint8_t* valid);
 int ensure_images(mocap_ctx* ctx, int n_images);
@@ -165,9 +174,21 @@ int blob_set_large_holes(mocap_ctx* ctx, int on);
 // candidate groups per work item of the chunked matcher: frame-sets with more are evaluated by several warps
 #define MOCAP_MATCH_CHUNK 512
 int launch_match_list(mocap_ctx* ctx, const int32_t* blob_xy, const int32_t* blob_n, const uint32_t* set_list, uint32_t* set_count,
-                      int n_sets_max, double* obj, double* err, int32_t* n_obj, int32_t* set_flags);
-int launch_pipeline_fused(mocap_ctx* ctx, const uint8_t* frames, int n_sets, int threshold,
-                          double* obj, double* err, int32_t* n_obj, int32_t* set_flags, int channels = 1);
+                      int n_sets_max, const SetOut& out, const int32_t* img_flags);
+int launch_pipeline_fused(mocap_ctx* ctx, const uint8_t* frames, int n_sets, int channels, int threshold, const SetOut& out);
+// S1-S3 of n_sets frame-sets through the single-pass kernel (fused) or the three-kernel pipeline, launch group by
+// launch group; frames_read (may be null) is recorded after the last launch that reads a group's frames (api.cu)
+int run_sets(mocap_ctx* ctx, const uint8_t* frames, int n_sets, int channels, int threshold, bool fused, const SetOut& out,
+             cudaEvent_t frames_read);
+bool pick_fused(const mocap_ctx* ctx);
+// the S1 launchers' shared pieces: the moment sums of a frame this size may exceed 32 bits (the kernels' WIDE variant);
+// mocap_enable_kernel_timing's event pair around the stream kernel (no-ops while timing is off); the pairs' read-out
+inline bool moments_wide(const mocap_config& c) {
+    const long long mx = c.width > c.height ? c.width : c.height;
+    return 6ll * mx * c.width * c.height >= (1ll << 32);
+}
+int timing_begin(mocap_ctx* ctx);
+int timing_end(mocap_ctx* ctx);
 int timing_flush(mocap_ctx* ctx);
 // cold-start pose chain (calib_init.cu): per adjacent pair an 8-point F started from init_inl (NULL = all common
 // observations) and re-fitted on its Sampson inliers at thr2, E, the cheirality vote and the chain

@@ -21,8 +21,7 @@ size_t fused_slab_bytes(const mocap_config& c) {
     return (m + 15) & ~(size_t)15;
 }
 
-int launch_pipeline_fused(mocap_ctx* ctx, const uint8_t* frames, int n_sets, int threshold,
-                          double* obj, double* err, int32_t* n_obj, int32_t* set_flags, int channels) {
+int launch_pipeline_fused(mocap_ctx* ctx, const uint8_t* frames, int n_sets, int channels, int threshold, const SetOut& out) {
     if (n_sets <= 0) return MOCAP_OK;
     const mocap_config& c = ctx->cfg;
     FusedParams P;
@@ -36,13 +35,7 @@ int launch_pipeline_fused(mocap_ctx* ctx, const uint8_t* frames, int n_sets, int
     P.units_per_image = (iters_total + 15) / 16;             // ~16 iterations (64 KB) per unit
     P.iters_per_unit = (iters_total + P.units_per_image - 1) / P.units_per_image;
     P.total_units = (long long)n_sets * c.n_cam * P.units_per_image;
-    if (threshold < 0) { P.tc.addc = 0x80808080u; P.tc.use_and = 0; }
-    else if (threshold >= 255) { P.tc.addc = 0; P.tc.use_and = 1; }
-    else {
-        const uint32_t T1 = (uint32_t)threshold + 1u;
-        P.tc.use_and = T1 > 128 ? 1u : 0u;
-        P.tc.addc = (T1 > 128 ? 256u - T1 : 128u - T1) * 0x01010101u;
-    }
+    P.tc = thresh_const(threshold);
     P.E = c.max_segments;
     P.seg_count = ctx->d_seg_count; P.seg_list = ctx->d_seg_list;
     P.img_done = ctx->d_img_done; P.set_done = ctx->d_set_done; P.set_defer = ctx->d_set_done + ctx->cap_images;
@@ -52,18 +45,14 @@ int launch_pipeline_fused(mocap_ctx* ctx, const uint8_t* frames, int n_sets, int
     P.set_worklist = ctx->d_set_worklist; P.set_work_count = ctx->d_work_count + 2;
     P.tb = ctx->d_tables;
     P.MB = c.max_blobs; P.RMAX = c.max_roots; P.KC = c.max_cands; P.GMAX = (uint32_t)c.max_groups;
-    P.obj = obj; P.err = err; P.n_obj = n_obj; P.set_flags = set_flags;
-    P.track_xy = ctx->track_xy_cur;
+    P.obj = out.obj; P.err = out.err; P.n_obj = out.n; P.set_flags = out.flags; P.track_xy = out.track_xy;
     P.slab_bytes = fused_slab_bytes(c);
     const size_t smem = P.slab_bytes * FUSED_WARPS;
-    const long long mx = c.width > c.height ? c.width : c.height;
-    const bool wide = 6ll * mx * c.width * c.height >= (1ll << 32);
+    const bool wide = moments_wide(c);
 
     CUDA_TRY(ctx, cudaMemsetAsync(ctx->d_unit_counter, 0, sizeof(unsigned long long), ctx->stream));
-    if (ctx->timing_on) {
-        if (ctx->tim_used == 64) { const int st = timing_flush(ctx); if (st) return st; }
-        CUDA_TRY(ctx, cudaEventRecord(ctx->tim_ev[2 * ctx->tim_used], ctx->stream));
-    }
+    int st = timing_begin(ctx);
+    if (st) return st;
     const int grid = ctx->num_sms * ctx->fused_ctas_per_sm;
     if (channels == 3) {                                     // H x W x 3 interleaved: the layout _find_dot receives
         if (wide) {
@@ -81,19 +70,13 @@ int launch_pipeline_fused(mocap_ctx* ctx, const uint8_t* frames, int n_sets, int
         else k_pipeline_fused<false, false><<<grid, FUSED_WARPS * 32, smem, ctx->stream>>>(P);
     }
     CUDA_TRY(ctx, cudaGetLastError());
-    if (ctx->timing_on) {
-        CUDA_TRY(ctx, cudaEventRecord(ctx->tim_ev[2 * ctx->tim_used + 1], ctx->stream));
-        ctx->tim_used += 1;
-    }
+    if ((st = timing_end(ctx)) != MOCAP_OK) return st;
     ctx->launches += 1;
     // slow path for whatever exceeded the warp-level capacities (normally nothing: both kernels
     // read an empty worklist and exit)
-    int st = launch_blob_fallback(ctx, ctx->d_blob_xy, ctx->d_blob_n, nullptr, ctx->d_img_flags, n_sets * ctx->cfg.n_cam);
-    if (st) return st;
-    st = launch_match_list(ctx, ctx->d_blob_xy, ctx->d_blob_n, ctx->d_set_worklist, ctx->d_work_count + 2, n_sets,
-                           obj, err, n_obj, set_flags);
-    if (st) return st;
-    return MOCAP_OK;
+    if ((st = launch_blob_fallback(ctx, ctx->d_blob_xy, ctx->d_blob_n, nullptr, ctx->d_img_flags, n_sets * ctx->cfg.n_cam)) != MOCAP_OK)
+        return st;
+    return launch_match_list(ctx, ctx->d_blob_xy, ctx->d_blob_n, ctx->d_set_worklist, ctx->d_work_count + 2, n_sets, out, ctx->d_img_flags);
 }
 
 int fused_kernel_init(mocap_ctx* ctx) {

@@ -133,8 +133,8 @@ static int ensure_match_split(mocap_ctx* ctx, int n_sets) {
     return st;
 }
 
-int launch_match(mocap_ctx* ctx, const int32_t* blob_xy, const int32_t* blob_n, int n_sets,
-                 double* obj, double* err, int32_t* n_obj, int32_t* set_flags, int32_t* chosen) {
+int launch_match(mocap_ctx* ctx, const int32_t* blob_xy, const int32_t* blob_n, int n_sets, const SetOut& out,
+                 const int32_t* img_flags, int32_t* chosen) {
     if (n_sets <= 0) return MOCAP_OK;
     const mocap_config& c = ctx->cfg;
     const int warps = 4;
@@ -155,13 +155,13 @@ int launch_match(mocap_ctx* ctx, const int32_t* blob_xy, const int32_t* blob_n, 
     CUDA_TRY(ctx, cudaMemsetAsync(ctx->match_counter.get(), 0, 4 * sizeof(unsigned), ctx->stream));
     k_match_triangulate<<<grid, warps * 32, smem, ctx->stream>>>(ctx->d_tables, blob_xy, blob_n, nullptr, nullptr, sp, n_sets, c.n_cam,
                                                                  c.max_blobs, c.max_roots, c.max_cands,
-                                                                 (uint32_t)c.max_groups, obj, err, n_obj, set_flags, chosen, ctx->track_xy_cur, ctx->img_flags_cur);
+                                                                 (uint32_t)c.max_groups, out.obj, out.err, out.n, out.flags, chosen, out.track_xy, img_flags);
     CUDA_TRY(ctx, cudaGetLastError());
     ctx->launches += 1;
     if (sp.items) {
         // how many items there are is known on the device only: a full persistent grid, warps without an item leave at once
         k_match_chunks<<<full, warps * 32, smem, ctx->stream>>>(ctx->d_tables, blob_xy, blob_n, sp, c.n_cam, c.max_blobs, c.max_roots, c.max_cands,
-                                                                (uint32_t)c.max_groups, obj, err, n_obj, set_flags, chosen, ctx->track_xy_cur, ctx->img_flags_cur);
+                                                                (uint32_t)c.max_groups, out.obj, out.err, out.n, out.flags, chosen, out.track_xy, img_flags);
         CUDA_TRY(ctx, cudaGetLastError());
         ctx->launches += 1;
     }
@@ -169,7 +169,7 @@ int launch_match(mocap_ctx* ctx, const int32_t* blob_xy, const int32_t* blob_n, 
 }
 
 int launch_match_list(mocap_ctx* ctx, const int32_t* blob_xy, const int32_t* blob_n, const uint32_t* set_list, uint32_t* set_count,
-                      int n_sets_max, double* obj, double* err, int32_t* n_obj, int32_t* set_flags) {
+                      int n_sets_max, const SetOut& out, const int32_t* img_flags) {
     const mocap_config& c = ctx->cfg;
     const int warps = 4;
     const size_t smem = match_smem_bytes(c, warps);
@@ -179,7 +179,7 @@ int launch_match_list(mocap_ctx* ctx, const int32_t* blob_xy, const int32_t* blo
     memset(&none, 0, sizeof(none));
     k_match_triangulate<<<grid, warps * 32, smem, ctx->stream>>>(ctx->d_tables, blob_xy, blob_n, set_list, set_count, none, n_sets_max, c.n_cam,
                                                                  c.max_blobs, c.max_roots, c.max_cands, (uint32_t)c.max_groups,
-                                                                 obj, err, n_obj, set_flags, nullptr, ctx->track_xy_cur, ctx->d_img_flags);
+                                                                 out.obj, out.err, out.n, out.flags, nullptr, out.track_xy, img_flags);
     CUDA_TRY(ctx, cudaGetLastError());
     ctx->launches += 1;
     return MOCAP_OK;

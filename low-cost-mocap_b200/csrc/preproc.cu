@@ -138,6 +138,7 @@ int run_raw_groups(mocap_ctx* ctx, const uint8_t* raw_frames, int n_frame_sets, 
     int st = grow_carved(ctx, ctx->scratch, Drain::stream, [&](Layout& L) { gray = L.take<uint8_t>((size_t)chunk * C * gray_bytes); });
     if (st) return st;
     if (stages == RAW_DETECT && (st = ensure_images(ctx, (n_frame_sets < chunk ? n_frame_sets : chunk) * C)) != MOCAP_OK) return st;
+    const SetOut sets{obj, err, n_obj, set_flags, nullptr};
     for (int s0 = 0; s0 < n_frame_sets; s0 += chunk) {
         const int ns = n_frame_sets - s0 < chunk ? n_frame_sets - s0 : chunk;
         uint8_t* out = processed ? processed + (size_t)s0 * C * gray_bytes * 3 : nullptr;
@@ -145,8 +146,7 @@ int run_raw_groups(mocap_ctx* ctx, const uint8_t* raw_frames, int n_frame_sets, 
                                stages == RAW_PREPROCESS ? nullptr : gray);
         if (st) return st;
         if (stages == RAW_MATCH)
-            st = mocap_pipeline_dev(ctx, gray, ns, 1, threshold, obj + (size_t)s0 * ctx->cfg.max_roots * 3, err + (size_t)s0 * ctx->cfg.max_roots,
-                                    n_obj + s0, set_flags ? set_flags + s0 : nullptr);
+            st = run_sets(ctx, gray, ns, 1, threshold, pick_fused(ctx), sets.at(ctx->cfg, s0), nullptr);
         else if (stages == RAW_DETECT)
             st = launch_detect(ctx, gray, ns * C, 1, threshold, ctx->d_blob_xy, ctx->d_blob_n, nullptr, ctx->d_img_flags);
         if (st) return st;

@@ -13,14 +13,7 @@ namespace {
 // the stream kernel's per-segment work (k_threshold_segments_c1), in a shuffled order: the kernel's atomic
 // append gives no order either
 std::vector<uint32_t> segments_of(const uint8_t* img, int W, int H, int threshold, unsigned seed) {
-    ThreshConst tc;
-    if (threshold < 0) { tc.addc = 0x80808080u; tc.use_and = 0; }
-    else if (threshold >= 255) { tc.addc = 0; tc.use_and = 1; }
-    else {
-        const uint32_t T1 = (uint32_t)threshold + 1u;
-        tc.use_and = T1 > 128 ? 1u : 0u;
-        tc.addc = (T1 > 128 ? 256u - T1 : 128u - T1) * 0x01010101u;
-    }
+    const ThreshConst tc = thresh_const(threshold);
     std::vector<uint32_t> list;
     const int n_seg = W * H / MOCAP_SEG_PX;
     for (int s = 0; s < n_seg; ++s) {

@@ -32,13 +32,7 @@ extern "C" int hc_pipeline_fused(const uint8_t* frames, int n_sets, int C, int W
     P.units_per_image = (iters_total + 15) / 16;
     P.iters_per_unit = (iters_total + P.units_per_image - 1) / P.units_per_image;
     P.total_units = (long long)n_sets * C * P.units_per_image;
-    if (threshold < 0) { P.tc.addc = 0x80808080u; P.tc.use_and = 0; }
-    else if (threshold >= 255) { P.tc.addc = 0; P.tc.use_and = 1; }
-    else {
-        const uint32_t T1 = (uint32_t)threshold + 1u;
-        P.tc.use_and = T1 > 128 ? 1u : 0u;
-        P.tc.addc = (T1 > 128 ? 256u - T1 : 128u - T1) * 0x01010101u;
-    }
+    P.tc = thresh_const(threshold);
     P.E = E;
     std::vector<uint32_t> seg_count(n_img, 0), seg_list((size_t)n_img * E, 0), img_done(n_img, 0), set_done(n_sets, 0), set_defer(n_sets, 0);
     std::vector<uint32_t> work_count(4, 0);

@@ -223,7 +223,8 @@ def test_batches_across_launch_groups(torch, monkeypatch):
     three-kernel pipeline) tiled from a pool of distinct frame-sets, the deferred ones placed on both sides of every
     group boundary and last: every frame-set equals the pool's own one-group result -- points, errors, counts, flags,
     winners' pixels -- in both pipelines, the two pipelines agree, and the device compaction of the whole batch's tracks
-    equals the concatenation of the per-set tracks."""
+    equals the concatenation of the per-set tracks.  The host entry point on a host copy of the batch (three staging
+    chunks of 24 966 frame-sets, each cut into seven launch groups by the three-kernel pipeline) equals it too."""
     C, H, W, P = 2, 48, 112, 40
     K = np.array([[100.0, 0, 56], [0, 100.0, 24], [0, 0, 1]])
     poses = [{"R": np.eye(3), "t": np.zeros(3)}, {"R": np.eye(3), "t": np.array([-0.2, 0.0, 0.0])}]
@@ -243,6 +244,7 @@ def test_batches_across_launch_groups(torch, monkeypatch):
         assert int(ref["flags"][0]) != 0 and int((ref["n"] > 0).sum()) > P // 2      # the 70-blob set overflows max_blobs
         big_in = pool_d[idx_d].contiguous()                                           # ~700 MB
         big = ctx.pipeline(big_in, want_tracks=True)
+        host = ctx.pipeline_host(big_in.cpu())
         del big_in
         torch.cuda.synchronize()
         R = ctx.cfg.max_roots
@@ -250,6 +252,9 @@ def test_batches_across_launch_groups(torch, monkeypatch):
         assert torch.equal(big["n"], ref["n"][idx_d]) and torch.equal(big["flags"], ref["flags"][idx_d]), mode
         for key in ("obj", "err", "track_xy"):
             assert torch.equal(big[key][live], ref[key][idx_d][live]), (mode, key)
+        assert torch.equal(host["n"], ref["n"][idx_d].cpu()) and torch.equal(host["flags"], ref["flags"][idx_d].cpu()), mode
+        for key in ("obj", "err"):
+            assert torch.equal(host[key][live.cpu()], ref[key][idx_d][live].cpu()), (mode, "host", key)
         obs = ctx.tracks_to_observations_dev(big)
         rows = ref["track_xy"][idx_d][live]                                           # [points, C, 2] in frame order
         mask = rows[..., 0] >= 0
