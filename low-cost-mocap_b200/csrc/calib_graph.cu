@@ -248,45 +248,33 @@ k_translation_residuals(const double* __restrict__ obs, const uint8_t* __restric
     front[idx] = fr;
 }
 
-static void hartley(const std::vector<float4>& pts, int o, int m, const std::vector<uint8_t>& inl, double T[6]) {
-    for (int side = 0; side < 2; ++side) {
-        double cx = 0, cy = 0; int k = 0;
-        for (int i = 0; i < m; ++i)
-            if (inl[o + i]) { const float4 v = pts[o + i]; cx += side ? v.z : v.x; cy += side ? v.w : v.y; ++k; }
-        cx /= k; cy /= k;
-        double md = 0;
-        for (int i = 0; i < m; ++i)
-            if (inl[o + i]) {
-                const float4 v = pts[o + i];
-                const double x = side ? v.z : v.x, y = side ? v.w : v.y;
-                md += sqrt((x - cx) * (x - cx) + (y - cy) * (y - cy));
-            }
-        md /= k;
-        const double sc = md > 0 ? sqrt(2.0) / md : 1.0;
-        T[3 * side] = sc; T[3 * side + 1] = -sc * cx; T[3 * side + 2] = -sc * cy;
-    }
+int fit_pairs(mocap_ctx* ctx, const PairTable& tab, const PairDev& d, const uint8_t* inl, double* F, uint8_t* ok) {
+    const int P = tab.pairs();
+    std::vector<double> hT(6 * (size_t)P), h45(45 * (size_t)P);
+    for (int p = 0; p < P; ++p)
+        calib_pose::hartley(reinterpret_cast<const float*>(&tab.pts[tab.off[p]]), tab.count(p), inl + tab.off[p], &hT[6 * p]);
+    cudaStream_t s = ctx->stream;
+    CUDA_TRY(ctx, cudaMemcpyAsync(d.T, hT.data(), hT.size() * 8, cudaMemcpyHostToDevice, s));
+    CUDA_TRY(ctx, cudaMemcpyAsync(d.inl, inl, tab.pts.size(), cudaMemcpyHostToDevice, s));
+    k_epipolar_normal_pairs<<<P, CG_THREADS, 0, s>>>(d.pts, d.off, d.inl, d.T, d.n45);
+    CUDA_TRY(ctx, cudaGetLastError());
+    ctx->launches += 1;
+    CUDA_TRY(ctx, cudaMemcpyAsync(h45.data(), d.n45, h45.size() * 8, cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(ctx, cudaStreamSynchronize(s));
+    for (int p = 0; p < P; ++p) ok[p] = calib_pose::fit_from_normal(&h45[45 * p], &hT[6 * p], F + 9 * p) ? 1 : 0;
+    return MOCAP_OK;
 }
 
-// F from the 45-entry normal matrix in normalised coordinates: smallest eigenvector, rank 2, de-normalised, unit norm
-// (the arithmetic of calib_init.cu's pair_motion)
-static bool fit_from_normal(const double* up, const double T[6], double F[9]) {
-    using namespace calib_pose;
-    std::vector<double> A(81), lam;
-    int k = 0;
-    for (int r = 0; r < 9; ++r) for (int c = r; c < 9; ++c) { A[9 * r + c] = up[k]; A[9 * c + r] = up[k]; ++k; }
-    if (!trf::sym_eig(9, A, lam)) return false;
-    int best = 0;
-    for (int i = 1; i < 9; ++i) if (lam[i] < lam[best]) best = i;
-    double Fn[9], U[9], sv[3], V[9], Fr[9], tmp[9];
-    for (int i = 0; i < 9; ++i) Fn[i] = A[9 * i + best];
-    svd3(Fn, U, sv, V);
-    for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) Fr[3 * i + j] = U[3 * i] * sv[0] * V[3 * j] + U[3 * i + 1] * sv[1] * V[3 * j + 1];
-    const double M1[9] = {T[0], 0, T[1], 0, T[0], T[2], 0, 0, 1}, M2t[9] = {T[3], 0, 0, 0, T[3], 0, T[4], T[5], 1};
-    mat3mul(M2t, Fr, tmp); mat3mul(tmp, M1, F);
-    double nf = 0; for (int i = 0; i < 9; ++i) nf += F[i] * F[i];
-    nf = sqrt(nf); if (nf > 0) for (int i = 0; i < 9; ++i) F[i] /= nf;
-    fix_sign(F);
-    return true;
+int select_pairs(mocap_ctx* ctx, const PairTable& tab, const PairDev& d, const double* F, double thr2, uint8_t* sel) {
+    const int P = tab.pairs();
+    cudaStream_t s = ctx->stream;
+    CUDA_TRY(ctx, cudaMemcpyAsync(d.F, F, (size_t)P * 9 * 8, cudaMemcpyHostToDevice, s));
+    k_sampson_pairs<<<dim3((tab.max_count() + CG_THREADS - 1) / CG_THREADS, P), CG_THREADS, 0, s>>>(d.pts, d.off, d.F, thr2, d.inl);
+    CUDA_TRY(ctx, cudaGetLastError());
+    ctx->launches += 1;
+    CUDA_TRY(ctx, cudaMemcpyAsync(sel, d.inl, tab.pts.size(), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(ctx, cudaStreamSynchronize(s));
+    return MOCAP_OK;
 }
 
 static void inv3(const double* K, double* Ki) {
@@ -335,24 +323,16 @@ extern "C" int mocap_calibrate_graph_host(mocap_ctx* ctx, const double* obs, con
                           "(0, 180] and irls_rounds in 1..64 (got %d, %d, %g, %g, %d)", who, go.min_common, go.min_inliers,
                           go.min_angle_deg, go.rot_outlier_deg, go.irls_rounds);
     // 1. pair table
-    std::vector<int> pa, pb, common;
-    std::vector<float4> pts;
-    std::vector<int> off(1, 0);
+    std::vector<int> pa, pb;
     for (int a = 0; a < C; ++a)
         for (int b = a + 1; b < C; ++b) {
             int m = 0;
             for (int f = 0; f < n_points; ++f) m += (mask[(size_t)f * C + a] && mask[(size_t)f * C + b]) ? 1 : 0;
-            if (m < go.min_common) continue;
-            pa.push_back(a); pb.push_back(b); common.push_back(m);
-            for (int f = 0; f < n_points; ++f)
-                if (mask[(size_t)f * C + a] && mask[(size_t)f * C + b]) {
-                    const double* xa = obs + ((size_t)f * C + a) * 2;
-                    const double* xb = obs + ((size_t)f * C + b) * 2;
-                    pts.push_back(make_float4((float)xa[0], (float)xa[1], (float)xb[0], (float)xb[1]));
-                }
-            off.push_back((int)pts.size());
+            if (m >= go.min_common) { pa.push_back(a); pb.push_back(b); }
         }
-    const int P = (int)pa.size();
+    const PairTable tab = pair_table(obs, mask, n_points, C, pa, pb);
+    const std::vector<int>& off = tab.off;
+    const int P = tab.pairs();
     {
         std::vector<uint8_t> all(P, 1);
         const unsigned lost = P ? cg_disconnected(C, P, pa.data(), pb.data(), all.data()) : ((1u << C) - 2u);
@@ -360,22 +340,21 @@ extern "C" int mocap_calibrate_graph_host(mocap_ctx* ctx, const double* obs, con
     }
     // 2. RANSAC over the pair table
     std::vector<double> F(9 * (size_t)P);
-    std::vector<uint8_t> inl(pts.size());
+    std::vector<uint8_t> inl(tab.pts.size());
     std::vector<unsigned long long> keys(P);
-    st = ransac_run(ctx, pts.data(), off.data(), P, ro, F.data(), inl.data(), keys.data());
+    st = ransac_run(ctx, tab, ro, F.data(), inl.data(), keys.data());
     if (st) { cudaGetLastError(); return st; }
     // device buffers of the later stages
-    const size_t total = pts.size(), nv = (size_t)n_points * C;
-    int mmax = 0;
-    for (int p = 0; p < P; ++p) mmax = std::max(mmax, off[p + 1] - off[p]);
+    const size_t total = tab.pts.size(), nv = (size_t)n_points * C;
+    const int mmax = tab.max_count();
     const int n3 = 3 * C, E = n3 * (n3 + 1) / 2;
     const int chunk = 64;
     const int G = (n_points + chunk - 1) / chunk;
-    float4* d_pts; int *d_off, *d_cnt; uint8_t *d_inl, *d_init, *d_front; CgCams* d_cams;
-    double *d_T, *d_45, *d_F, *d_cand, *d_ang, *d_obs, *d_w[2], *d_t, *d_part, *d_H;
+    PairDev d;
+    int* d_cnt; uint8_t *d_init, *d_front; CgCams* d_cams;
+    double *d_cand, *d_ang, *d_obs, *d_w[2], *d_t, *d_part, *d_H;
     st = grow_carved(ctx, ctx->scratch, Drain::stream, [&](Layout& L) {
-        d_pts = L.take<float4>(total); d_off = L.take<int>(P + 1); d_inl = L.take<uint8_t>(total);
-        d_T = L.take<double>((size_t)P * 6); d_45 = L.take<double>((size_t)P * 45); d_F = L.take<double>((size_t)P * 9);
+        d.take(L, tab);
         d_cand = L.take<double>((size_t)P * 4 * CG_CAND); d_cnt = L.take<int>((size_t)P * 4); d_ang = L.take<double>(total * 4);
         d_obs = L.take<double>(nv * 2); d_init = L.take<uint8_t>(nv); d_w[0] = L.take<double>(nv); d_w[1] = L.take<double>(nv);
         d_front = L.take<uint8_t>(nv); d_cams = L.take<CgCams>(1);
@@ -383,12 +362,12 @@ extern "C" int mocap_calibrate_graph_host(mocap_ctx* ctx, const double* obs, con
     });
     if (st) { cudaGetLastError(); return st; }
     cudaStream_t s = ctx->stream;
-    CUDA_TRY(ctx, cudaMemcpyAsync(d_pts, pts.data(), total * sizeof(float4), cudaMemcpyHostToDevice, s));
-    CUDA_TRY(ctx, cudaMemcpyAsync(d_off, off.data(), (P + 1) * sizeof(int), cudaMemcpyHostToDevice, s));
+    CUDA_TRY(ctx, cudaMemcpyAsync(d.pts, tab.pts.data(), total * sizeof(float4), cudaMemcpyHostToDevice, s));
+    CUDA_TRY(ctx, cudaMemcpyAsync(d.off, off.data(), (P + 1) * sizeof(int), cudaMemcpyHostToDevice, s));
     // 3. re-fits: three 8-point fits, each followed by a Sampson re-selection at the RANSAC threshold; the last
     //    selection is the pair's inlier set.  A pair without a model, or whose selection falls under 8 points, keeps
     //    its previous set.
-    std::vector<uint8_t> ok(P);
+    std::vector<uint8_t> ok(P), fitted(P);
     for (int p = 0; p < P; ++p) {
         ok[p] = keys[p] ? 1 : 0;
         int k = 0;
@@ -396,25 +375,11 @@ extern "C" int mocap_calibrate_graph_host(mocap_ctx* ctx, const double* obs, con
         if (k < 8) for (int i = off[p]; i < off[p + 1]; ++i) inl[i] = 1;
     }
     const double thr2 = ro.threshold_px * ro.threshold_px;
-    std::vector<double> hT(6 * (size_t)P), h45(45 * (size_t)P);
     std::vector<uint8_t> sel(total);
     for (int round = 0; round < 3; ++round) {
-        for (int p = 0; p < P; ++p) hartley(pts, off[p], off[p + 1] - off[p], inl, &hT[6 * p]);
-        CUDA_TRY(ctx, cudaMemcpyAsync(d_T, hT.data(), hT.size() * 8, cudaMemcpyHostToDevice, s));
-        CUDA_TRY(ctx, cudaMemcpyAsync(d_inl, inl.data(), total, cudaMemcpyHostToDevice, s));
-        k_epipolar_normal_pairs<<<P, CG_THREADS, 0, s>>>(d_pts, d_off, d_inl, d_T, d_45);
-        CUDA_TRY(ctx, cudaGetLastError());
-        ctx->launches += 1;
-        CUDA_TRY(ctx, cudaMemcpyAsync(h45.data(), d_45, h45.size() * 8, cudaMemcpyDeviceToHost, s));
-        CUDA_TRY(ctx, cudaStreamSynchronize(s));
-        for (int p = 0; p < P; ++p)
-            if (!fit_from_normal(&h45[45 * p], &hT[6 * p], &F[9 * p])) ok[p] = 0;
-        CUDA_TRY(ctx, cudaMemcpyAsync(d_F, F.data(), F.size() * 8, cudaMemcpyHostToDevice, s));
-        k_sampson_pairs<<<dim3((mmax + CG_THREADS - 1) / CG_THREADS, P), CG_THREADS, 0, s>>>(d_pts, d_off, d_F, thr2, d_inl);
-        CUDA_TRY(ctx, cudaGetLastError());
-        ctx->launches += 1;
-        CUDA_TRY(ctx, cudaMemcpyAsync(sel.data(), d_inl, total, cudaMemcpyDeviceToHost, s));
-        CUDA_TRY(ctx, cudaStreamSynchronize(s));
+        if ((st = fit_pairs(ctx, tab, d, inl.data(), F.data(), fitted.data()))) return st;
+        for (int p = 0; p < P; ++p) ok[p] &= fitted[p];
+        if ((st = select_pairs(ctx, tab, d, F.data(), thr2, sel.data()))) return st;
         for (int p = 0; p < P; ++p) {
             int k = 0;
             for (int i = off[p]; i < off[p + 1]; ++i) k += sel[i];
@@ -442,9 +407,9 @@ extern "C" int mocap_calibrate_graph_host(mocap_ctx* ctx, const double* obs, con
     std::vector<int> counts((size_t)P * 4);
     std::vector<double> ang(total * 4);
     CUDA_TRY(ctx, cudaMemcpyAsync(d_cand, cand.data(), cand.size() * 8, cudaMemcpyHostToDevice, s));
-    CUDA_TRY(ctx, cudaMemcpyAsync(d_inl, inl.data(), total, cudaMemcpyHostToDevice, s));
+    CUDA_TRY(ctx, cudaMemcpyAsync(d.inl, inl.data(), total, cudaMemcpyHostToDevice, s));
     CUDA_TRY(ctx, cudaMemsetAsync(d_cnt, 0, (size_t)P * 4 * sizeof(int), s));
-    k_pair_cheirality<<<dim3((4 * mmax + CG_THREADS - 1) / CG_THREADS, P), CG_THREADS, 0, s>>>(d_pts, d_off, d_inl, d_cand, d_cnt, d_ang);
+    k_pair_cheirality<<<dim3((4 * mmax + CG_THREADS - 1) / CG_THREADS, P), CG_THREADS, 0, s>>>(d.pts, d.off, d.inl, d_cand, d_cnt, d_ang);
     CUDA_TRY(ctx, cudaGetLastError());
     ctx->launches += 1;
     CUDA_TRY(ctx, cudaMemcpyAsync(counts.data(), d_cnt, counts.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
@@ -455,7 +420,7 @@ extern "C" int mocap_calibrate_graph_host(mocap_ctx* ctx, const double* obs, con
     std::vector<uint8_t> use(P, 0);
     for (int p = 0; p < P; ++p) {
         mocap_graph_pair& r = rep[p];
-        r.a = pa[p]; r.b = pb[p]; r.common = common[p];
+        r.a = pa[p]; r.b = pb[p]; r.common = tab.count(p);
         r.inliers = 0;
         for (int i = off[p]; i < off[p + 1]; ++i) r.inliers += inl[i];
         int best = -1, bc = 0;

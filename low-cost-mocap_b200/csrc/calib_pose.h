@@ -1,7 +1,11 @@
-// Host 3x3 algebra of the cold-start calibration (calib_init.cu, calib_graph.cu and the g++ host checks): symmetric
-// eigen-decomposition, SVD, and libmv's MotionFromEssential.  Plain C++, no CUDA.
+// Host algebra of the cold-start calibration (calib_init.cu, calib_graph.cu and the g++ host checks): symmetric 3x3
+// eigen-decomposition, SVD, libmv's MotionFromEssential, and the normalised 8-point fit's Hartley transform and solve.
+// Plain C++, no CUDA.
 #pragma once
 #include <math.h>
+#include <stdint.h>
+#include <vector>
+#include "trf_core.h"
 
 namespace calib_pose {
 
@@ -91,6 +95,49 @@ inline void motion_from_essential(const double E[9], double Rs[4][9], double ts[
     mat3mul(U, Wt, UWt); mat3mul(UWt, Vt, Bm);
     for (int k = 0; k < 9; ++k) { Rs[0][k] = A[k]; Rs[1][k] = A[k]; Rs[2][k] = Bm[k]; Rs[3][k] = Bm[k]; }
     for (int r = 0; r < 3; ++r) { ts[0][r] = U[3 * r + 2]; ts[1][r] = -U[3 * r + 2]; ts[2][r] = U[3 * r + 2]; ts[3][r] = -U[3 * r + 2]; }
+}
+
+// Hartley normalisation of a pair's fit set: pts [m][4] {x_a, y_a, x_b, y_b}, inl [m] the set (not empty).  T = {s_a,
+// tx_a, ty_a, s_b, tx_b, ty_b}: per view x' = s x + tx, y' = s y + ty moves the set's centroid to 0 and its mean
+// distance from it to sqrt(2).
+inline void hartley(const float* pts, int m, const uint8_t* inl, double T[6]) {
+    for (int side = 0; side < 2; ++side) {
+        double cx = 0, cy = 0; int k = 0;
+        for (int i = 0; i < m; ++i)
+            if (inl[i]) { cx += pts[4 * i + 2 * side]; cy += pts[4 * i + 2 * side + 1]; ++k; }
+        cx /= k; cy /= k;
+        double md = 0;
+        for (int i = 0; i < m; ++i)
+            if (inl[i]) {
+                const double x = pts[4 * i + 2 * side], y = pts[4 * i + 2 * side + 1];
+                md += sqrt((x - cx) * (x - cx) + (y - cy) * (y - cy));
+            }
+        md /= k;
+        const double sc = md > 0 ? sqrt(2.0) / md : 1.0;
+        T[3 * side] = sc; T[3 * side + 1] = -sc * cx; T[3 * side + 2] = -sc * cy;
+    }
+}
+
+// F (x_b^T F x_a = 0) from the 45-entry upper triangle of the 8-point normal matrix in the coordinates of hartley()'s T:
+// smallest eigenvector, rank 2, de-normalised, unit norm, fix_sign.  False (F untouched) if the eigen problem fails.
+inline bool fit_from_normal(const double* up, const double T[6], double F[9]) {
+    std::vector<double> A(81), lam;
+    int k = 0;
+    for (int r = 0; r < 9; ++r) for (int c = r; c < 9; ++c) { A[9 * r + c] = up[k]; A[9 * c + r] = up[k]; ++k; }
+    if (!trf::sym_eig(9, A, lam)) return false;
+    int best = 0;
+    for (int i = 1; i < 9; ++i) if (lam[i] < lam[best]) best = i;
+    double Fn[9], U[9], sv[3], V[9], Fr[9], tmp[9];
+    for (int i = 0; i < 9; ++i) Fn[i] = A[9 * i + best];
+    svd3(Fn, U, sv, V);
+    for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) Fr[3 * i + j] = U[3 * i] * sv[0] * V[3 * j] + U[3 * i + 1] * sv[1] * V[3 * j + 1];
+    // F = T_b^T Fr T_a with T = [[s,0,tx],[0,s,ty],[0,0,1]]
+    const double M1[9] = {T[0], 0, T[1], 0, T[0], T[2], 0, 0, 1}, M2t[9] = {T[3], 0, 0, 0, T[3], 0, T[4], T[5], 1};
+    mat3mul(M2t, Fr, tmp); mat3mul(tmp, M1, F);
+    double nf = 0; for (int i = 0; i < 9; ++i) nf += F[i] * F[i];
+    nf = sqrt(nf); if (nf > 0) for (int i = 0; i < 9; ++i) F[i] /= nf;
+    fix_sign(F);
+    return true;
 }
 
 }  // namespace calib_pose

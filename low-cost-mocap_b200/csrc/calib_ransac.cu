@@ -98,11 +98,10 @@ int ransac_check_options(mocap_ctx* ctx, const mocap_ransac_options* opt, mocap_
     return MOCAP_OK;
 }
 
-int ransac_run(mocap_ctx* ctx, const float4* h_pts, const int* h_off, int P, const mocap_ransac_options& o, double* F_best,
-               uint8_t* inl, unsigned long long* keys) {
-    const int H = o.hypotheses;
+int ransac_run(mocap_ctx* ctx, const PairTable& tab, const mocap_ransac_options& o, double* F_best, uint8_t* inl, unsigned long long* keys) {
+    const int H = o.hypotheses, P = tab.pairs();
     const double thr2 = o.threshold_px * o.threshold_px;
-    const size_t total = (size_t)h_off[P];
+    const size_t total = tab.pts.size();
     CUDA_TRY(ctx, cudaSetDevice(ctx->cfg.device));
     float4* d_pts; int *d_off, *d_n; double *d_models, *d_F; unsigned long long* d_best; uint8_t* d_inl;
     int st = grow_carved(ctx, ctx->scratch, Drain::stream, [&](Layout& L) {
@@ -112,8 +111,8 @@ int ransac_run(mocap_ctx* ctx, const float4* h_pts, const int* h_off, int P, con
     });
     if (st) return st;
     cudaStream_t s = ctx->stream;
-    CUDA_TRY(ctx, cudaMemcpyAsync(d_pts, h_pts, total * sizeof(float4), cudaMemcpyHostToDevice, s));
-    CUDA_TRY(ctx, cudaMemcpyAsync(d_off, h_off, (P + 1) * sizeof(int), cudaMemcpyHostToDevice, s));
+    CUDA_TRY(ctx, cudaMemcpyAsync(d_pts, tab.pts.data(), total * sizeof(float4), cudaMemcpyHostToDevice, s));
+    CUDA_TRY(ctx, cudaMemcpyAsync(d_off, tab.off.data(), (P + 1) * sizeof(int), cudaMemcpyHostToDevice, s));
     CUDA_TRY(ctx, cudaMemsetAsync(d_best, 0, P * sizeof(unsigned long long), s));
     k_ransac_hypotheses<<<dim3((H + RS_HYP_THREADS - 1) / RS_HYP_THREADS, P), RS_HYP_THREADS, 0, s>>>(
         d_pts, d_off, H, (unsigned long long)o.seed, d_models, d_n);
@@ -121,7 +120,7 @@ int ransac_run(mocap_ctx* ctx, const float4* h_pts, const int* h_off, int P, con
     k_ransac_score<<<dim3((H + RS_SCORE_WARPS - 1) / RS_SCORE_WARPS, P), RS_SCORE_WARPS * 32, 0, s>>>(d_pts, d_off, H, thr2, d_models,
                                                                                                       d_n, d_best);
     CUDA_TRY(ctx, cudaGetLastError());
-    const int mmax = [&] { int x = 0; for (int c = 0; c < P; ++c) x = h_off[c + 1] - h_off[c] > x ? h_off[c + 1] - h_off[c] : x; return x; }();
+    const int mmax = tab.max_count();
     k_ransac_mask<<<dim3((mmax + 255) / 256 < 32 ? (mmax + 255) / 256 : 32, P), 256, 0, s>>>(d_pts, d_off, H, thr2, d_models, d_best,
                                                                                             d_inl, d_F);
     CUDA_TRY(ctx, cudaGetLastError());
@@ -133,32 +132,52 @@ int ransac_run(mocap_ctx* ctx, const float4* h_pts, const int* h_off, int P, con
     return MOCAP_OK;
 }
 
-// RANSAC over every adjacent pair: F_best [C-1][9] and, per pair, the inlier mask over its common observations in
-// frame order (inl, pair after pair; off [C] gives each pair's start).  Pair p is cameras (p, p+1).  Validates
+PairTable pair_table(const double* obs, const uint8_t* mask, int n_points, int C, const std::vector<int>& a, const std::vector<int>& b) {
+    PairTable tab{a, b, {}, {0}};
+    for (size_t k = 0; k < a.size(); ++k) {
+        for (int f = 0; f < n_points; ++f)
+            if (mask[(size_t)f * C + a[k]] && mask[(size_t)f * C + b[k]]) {      // index.py:242-244
+                const double* xa = obs + ((size_t)f * C + a[k]) * 2;
+                const double* xb = obs + ((size_t)f * C + b[k]) * 2;
+                tab.pts.push_back(make_float4((float)xa[0], (float)xa[1], (float)xb[0], (float)xb[1]));
+            }
+        tab.off.push_back((int)tab.pts.size());
+    }
+    return tab;
+}
+
+int adjacent_pairs(mocap_ctx* ctx, const double* obs, const uint8_t* mask, int n_points, const char* who, PairTable& tab) {
+    const int C = ctx->cfg.n_cam;
+    std::vector<int> a, b;
+    for (int c = 0; c + 1 < C; ++c) { a.push_back(c); b.push_back(c + 1); }
+    tab = pair_table(obs, mask, n_points, C, a, b);
+    for (int c = 0; c + 1 < C; ++c)
+        if (tab.count(c) < 8) return mocap_fail(ctx, MOCAP_EINVAL, "%s: cameras %d and %d share only %d observations", who, c, c + 1, tab.count(c));
+    return MOCAP_OK;
+}
+
+void scatter_pairs(const PairTable& tab, const uint8_t* mask, int n_points, int C, const uint8_t* sel, uint8_t* out) {
+    const int P = tab.pairs();
+    memset(out, 0, (size_t)n_points * P);
+    for (int p = 0; p < P; ++p)
+        for (int f = 0, k = tab.off[p]; f < n_points; ++f)
+            if (mask[(size_t)f * C + tab.a[p]] && mask[(size_t)f * C + tab.b[p]]) out[(size_t)f * P + p] = sel[k++];
+}
+
+// RANSAC over every adjacent pair: F_best [C-1][9], the adjacent table and the inlier mask over it.  Validates
 // everything before any launch.
 static int ransac_pairs(mocap_ctx* ctx, const double* obs, const uint8_t* mask, int n_points, const mocap_ransac_options* opt,
-                 double* F_best, std::vector<uint8_t>& inl, std::vector<int>& off, const char* who) {
+                        double* F_best, std::vector<uint8_t>& inl, PairTable& tab, const char* who) {
     const int C = ctx->cfg.n_cam, P = C - 1;
     if (!obs || !mask || n_points < 8 || C < 2) return mocap_fail(ctx, MOCAP_EINVAL, "%s: bad argument", who);
     mocap_ransac_options o;
     int st = ransac_check_options(ctx, opt, &o, who);
     if (st) return st;
-    std::vector<float4> pts;
-    off.assign(C, 0);
-    for (int c = 0; c < P; ++c) {
-        off[c] = (int)pts.size();
-        for (int f = 0; f < n_points; ++f)
-            if (mask[(size_t)f * C + c] && mask[(size_t)f * C + c + 1]) {      // index.py:242-244
-                const double* a = obs + ((size_t)f * C + c) * 2;
-                pts.push_back(make_float4((float)a[0], (float)a[1], (float)a[2], (float)a[3]));
-            }
-        const int m = (int)pts.size() - off[c];
-        if (m < 8) return mocap_fail(ctx, MOCAP_EINVAL, "%s: cameras %d and %d share only %d observations", who, c, c + 1, m);
-    }
-    off[P] = (int)pts.size();
+    st = adjacent_pairs(ctx, obs, mask, n_points, who, tab);
+    if (st) return st;
     std::vector<unsigned long long> keys(P);
-    inl.resize(pts.size());
-    st = ransac_run(ctx, pts.data(), off.data(), P, o, F_best, inl.data(), keys.data());
+    inl.resize(tab.pts.size());
+    st = ransac_run(ctx, tab, o, F_best, inl.data(), keys.data());
     if (st) return st;
     for (int c = 0; c < P; ++c)
         if (!keys[c]) return mocap_fail(ctx, MOCAP_EINVAL, "%s: no 7-point sample of cameras %d and %d gave a model", who, c, c + 1);
@@ -177,16 +196,10 @@ extern "C" int mocap_fundamental_ransac_host(mocap_ctx* ctx, const double* obs, 
     if (!ctx) return MOCAP_EINVAL;
     if (!F) return mocap_fail(ctx, MOCAP_EINVAL, "mocap_fundamental_ransac_host: bad argument");
     std::vector<uint8_t> inl;
-    std::vector<int> off;
-    const int st = ransac_pairs(ctx, obs, mask, n_points, opt, F, inl, off, "mocap_fundamental_ransac_host");
+    PairTable tab;
+    const int st = ransac_pairs(ctx, obs, mask, n_points, opt, F, inl, tab, "mocap_fundamental_ransac_host");
     if (st) return st;
-    if (inliers) {
-        const int C = ctx->cfg.n_cam;
-        memset(inliers, 0, (size_t)n_points * (C - 1));
-        for (int c = 0; c + 1 < C; ++c)
-            for (int f = 0, k = off[c]; f < n_points; ++f)
-                if (mask[(size_t)f * C + c] && mask[(size_t)f * C + c + 1]) inliers[(size_t)f * (C - 1) + c] = inl[k++];
-    }
+    if (inliers) scatter_pairs(tab, mask, n_points, ctx->cfg.n_cam, inl.data(), inliers);
     return MOCAP_OK;
 }
 
@@ -198,9 +211,9 @@ extern "C" int mocap_calibrate_init_ransac_host(mocap_ctx* ctx, const double* ob
     if (!ctx->cameras_set) return mocap_fail(ctx, MOCAP_ESTATE, "mocap_set_cameras has not been called (intrinsics are needed)");
     std::vector<double> F_best(9 * (size_t)(ctx->cfg.n_cam > 1 ? ctx->cfg.n_cam - 1 : 1));
     std::vector<uint8_t> inl;
-    std::vector<int> off;
-    int st = ransac_pairs(ctx, obs, mask, n_points, opt, F_best.data(), inl, off, "mocap_calibrate_init_ransac_host");
+    PairTable tab;
+    int st = ransac_pairs(ctx, obs, mask, n_points, opt, F_best.data(), inl, tab, "mocap_calibrate_init_ransac_host");
     if (st) return st;
     const double thr = opt ? opt->threshold_px : 1.0;
-    return calibrate_chain(ctx, obs, mask, n_points, nullptr, inl.data(), thr * thr, R, t, F_used, votes, inliers);
+    return calibrate_chain(ctx, tab, mask, n_points, nullptr, inl.data(), thr * thr, R, t, F_used, votes, inliers);
 }

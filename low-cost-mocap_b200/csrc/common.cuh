@@ -4,6 +4,7 @@
 #include <stdint.h>
 #include <stdio.h>
 #include <string.h>
+#include <vector>
 #include "../../include/mocap_b200.h"
 #include "ctx_memory.h"
 
@@ -190,15 +191,45 @@ inline bool moments_wide(const mocap_config& c) {
 int timing_begin(mocap_ctx* ctx);
 int timing_end(mocap_ctx* ctx);
 int timing_flush(mocap_ctx* ctx);
-// cold-start pose chain (calib_init.cu): per adjacent pair an 8-point F started from init_inl (NULL = all common
-// observations) and re-fitted on its Sampson inliers at thr2, E, the cheirality vote and the chain
-int calibrate_chain(mocap_ctx* ctx, const double* obs, const uint8_t* mask, int n_points, const double* F_given,
+// The cold-start calibration's pair table (calib_ransac.cu): for camera pairs (a[k], b[k]) their common observations
+// {x_a, y_a, x_b, y_b} in frame order, cast to float32 as the reference casts them (index.py:243-244), pair k at
+// [off[k], off[k+1]).  adjacent_pairs: the chain's table, pairs (c, c+1), failing with MOCAP_EINVAL where a pair has
+// fewer than 8 common observations.  scatter_pairs: a mask over the table -> out [n_points][P], 0 where a frame is not
+// common to the pair.
+struct PairTable {
+    std::vector<int> a, b;
+    std::vector<float4> pts;
+    std::vector<int> off;
+    int pairs() const { return (int)a.size(); }
+    int count(int k) const { return off[k + 1] - off[k]; }
+    int max_count() const { int x = 0; for (int k = 0; k < pairs(); ++k) x = count(k) > x ? count(k) : x; return x; }
+};
+PairTable pair_table(const double* obs, const uint8_t* mask, int n_points, int C, const std::vector<int>& a, const std::vector<int>& b);
+int adjacent_pairs(mocap_ctx* ctx, const double* obs, const uint8_t* mask, int n_points, const char* who, PairTable& tab);
+void scatter_pairs(const PairTable& tab, const uint8_t* mask, int n_points, int C, const uint8_t* sel, uint8_t* out);
+// cold-start pose chain over the adjacent table (calib_init.cu): per pair an 8-point F started from init_inl (over the
+// table; NULL = all common observations) and re-fitted on its Sampson inliers at thr2, E, the cheirality vote and the
+// chain; inl_out (may be NULL) [n_points][C-1] the final Sampson sets
+int calibrate_chain(mocap_ctx* ctx, const PairTable& tab, const uint8_t* mask, int n_points, const double* F_given,
                     const uint8_t* init_inl, double thr2, double* R, double* t, double* F_used, int* votes, uint8_t* inl_out);
-// RANSAC fundamental matrices over a list of camera pairs (calib_ransac.cu).  ransac_check_options fills o (opt NULL =
-// defaults) or fails with MOCAP_EINVAL.  ransac_run: h_pts holds every pair's common observations {x_a, y_a, x_b, y_b}
-// (float32), pair p at [h_off[p], h_off[p+1]); pair p's samples are drawn from the hash of (seed, p, ...).  Out: F_best
-// [P][9], inl over h_pts, keys [P] (0: no sample of that pair gave a model).  Three launches, one synchronisation.
+// RANSAC fundamental matrices over a pair table (calib_ransac.cu).  ransac_check_options fills o (opt NULL = defaults) or
+// fails with MOCAP_EINVAL.  ransac_run: pair p's samples are drawn from the hash of (seed, p, ...).  Out: F_best [P][9],
+// inl over the table, keys [P] (0: no sample of that pair gave a model).  Three launches, one synchronisation.
 // Scratch: dominated by P * hypotheses * 27 doubles of models.
 int ransac_check_options(mocap_ctx* ctx, const mocap_ransac_options* opt, mocap_ransac_options* o, const char* who);
-int ransac_run(mocap_ctx* ctx, const float4* h_pts, const int* h_off, int P, const mocap_ransac_options& o, double* F_best,
-               uint8_t* inl, unsigned long long* keys);
+int ransac_run(mocap_ctx* ctx, const PairTable& tab, const mocap_ransac_options& o, double* F_best, uint8_t* inl, unsigned long long* keys);
+// The 8-point re-fits of every pair of a table at once (calib_graph.cu).  PairDev: the table on the device and the
+// stages' buffers, carved by take(); the caller copies pts and off up.  fit_pairs: per pair the Hartley transform of
+// its fit set inl (host, over the table), k_epipolar_normal_pairs, calib_pose::fit_from_normal; F [P][9] (host) is
+// overwritten where ok[p] = 1 and left where the eigen problem fails.  select_pairs: k_sampson_pairs under F at thr2,
+// the selection sel (host, over the table) out.  One launch and one synchronisation each.
+struct PairDev {
+    float4* pts; int* off; uint8_t* inl; double *T, *n45, *F;
+    void take(Layout& L, const PairTable& tab) {
+        const size_t P = tab.pairs(), total = tab.pts.size();
+        pts = L.take<float4>(total); off = L.take<int>(P + 1); inl = L.take<uint8_t>(total);
+        T = L.take<double>(P * 6); n45 = L.take<double>(P * 45); F = L.take<double>(P * 9);
+    }
+};
+int fit_pairs(mocap_ctx* ctx, const PairTable& tab, const PairDev& d, const uint8_t* inl, double* F, uint8_t* ok);
+int select_pairs(mocap_ctx* ctx, const PairTable& tab, const PairDev& d, const double* F, double thr2, uint8_t* sel);

@@ -101,7 +101,7 @@ def ransac_models(libs, pts, pair, H, seed, thr):
 
 # ------------------------------------------------------------------------------------------------------------ 8-point
 def hartley(q, inl):
-    """(s, tx, ty) of the Hartley normalisation of q [m, 2] over the set inl, as hartley() / pair_motion form it."""
+    """(s, tx, ty) of the Hartley normalisation of q [m, 2] over the set inl, as calib_pose::hartley forms it."""
     h = q[inl]
     cx, cy = h[:, 0].sum() / len(h), h[:, 1].sum() / len(h)
     md = np.sqrt((h[:, 0] - cx) ** 2 + (h[:, 1] - cy) ** 2).sum() / len(h)
@@ -134,7 +134,8 @@ def fit_numpy(x1, x2, inl, T):
 
 
 def fit_product(libs):
-    """The product's host fit (hc_fit_from_normal: trf::sym_eig and svd3, the product's sign) on the numpy normal matrix."""
+    """The product's host fit (hc_fit_from_normal calls calib_pose::fit_from_normal: trf::sym_eig and svd3, the
+    product's sign) on the numpy normal matrix."""
     def fit(x1, x2, inl, T):
         F = np.zeros(9)
         assert libs.cg.hc_fit_from_normal(ptr(normal45(x1, x2, inl, T)), ptr(c64(T)), ptr(F)) == 1
@@ -143,7 +144,7 @@ def fit_product(libs):
 
 
 def sampson(F, x1, x2):
-    """Sampson distance^2 of k_sampson_inliers / k_sampson_pairs, in float64."""
+    """Sampson distance^2 of k_sampson_pairs, in float64."""
     F = np.asarray(F).ravel()
     l0 = F[0] * x1[:, 0] + F[1] * x1[:, 1] + F[2]
     l1 = F[3] * x1[:, 0] + F[4] * x1[:, 1] + F[5]
@@ -155,10 +156,10 @@ def sampson(F, x1, x2):
 
 
 def chain_refit(x1, x2, inl0, thr2, fit=fit_numpy):
-    """calib_init.cu's pair_motion estimator from the fit set inl0 (None: all points; a set of fewer than 8 falls back
-    to all): three fits, each but the last followed by a Sampson selection at thr2 that becomes the next fit set (all
-    points when it holds fewer than 8); a selection of every point after the second fit ends the rounds.  Returns
-    (F, final set, smallest relative Sampson margin)."""
+    """calibrate_chain's estimator (calib_init.cu) for one pair from the fit set inl0 (None: all points; a set of fewer
+    than 8 falls back to all): three fits, each but the last followed by a Sampson selection at thr2 that becomes the
+    next fit set (all points when it holds fewer than 8); a selection of every point after the second fit ends the
+    pair's rounds.  Returns (F, final set, smallest relative Sampson margin)."""
     n = len(x1)
     inl = np.ones(n, dtype=bool)
     if inl0 is not None and inl0.sum() >= 8:
@@ -181,7 +182,7 @@ def chain_refit(x1, x2, inl0, thr2, fit=fit_numpy):
 
 
 def eight_point_refit(x1, x2, inl0, thr=1.0):
-    """numpy restatement of calib_init.cu's pair_motion estimator started from a given fit set: normalised 8-point,
+    """numpy restatement of calibrate_chain's estimator (calib_init.cu) started from a given fit set: normalised 8-point,
     rank 2, then re-fits on the Sampson inliers, three fits in all.  F up to sign."""
     return chain_refit(np.asarray(x1, dtype=np.float64), np.asarray(x2, dtype=np.float64), np.asarray(inl0, dtype=bool), thr * thr)[0]
 

@@ -77,28 +77,9 @@ void hc_cheirality_pair(const double* Ka, const double* Kb, const double* R, con
     }
 }
 
-// F from the 45-entry upper triangle of a normal matrix in normalised coordinates and T = {s1, tx1, ty1, s2, tx2, ty2}:
-// the arithmetic of fit_from_normal (calib_graph.cu) and of pair_motion (calib_init.cu) -- smallest eigenvector by
-// trf::sym_eig, rank 2 by svd3, de-normalised, unit norm, with the product's sign.  Returns 0 if the eigen problem fails.
-int hc_fit_from_normal(const double* up, const double* T, double* F) {
-    using namespace calib_pose;
-    std::vector<double> A(81), lam;
-    int k = 0;
-    for (int r = 0; r < 9; ++r) for (int c = r; c < 9; ++c) { A[9 * r + c] = up[k]; A[9 * c + r] = up[k]; ++k; }
-    if (!trf::sym_eig(9, A, lam)) return 0;
-    int best = 0;
-    for (int i = 1; i < 9; ++i) if (lam[i] < lam[best]) best = i;
-    double Fn[9], U[9], sv[3], V[9], Fr[9], tmp[9];
-    for (int i = 0; i < 9; ++i) Fn[i] = A[9 * i + best];
-    svd3(Fn, U, sv, V);
-    for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) Fr[3 * i + j] = U[3 * i] * sv[0] * V[3 * j] + U[3 * i + 1] * sv[1] * V[3 * j + 1];
-    const double M1[9] = {T[0], 0, T[1], 0, T[0], T[2], 0, 0, 1}, M2t[9] = {T[3], 0, 0, 0, T[3], 0, T[4], T[5], 1};
-    mat3mul(M2t, Fr, tmp); mat3mul(tmp, M1, F);
-    double nf = 0; for (int i = 0; i < 9; ++i) nf += F[i] * F[i];
-    nf = sqrt(nf); if (nf > 0) for (int i = 0; i < 9; ++i) F[i] /= nf;
-    fix_sign(F);
-    return 1;
-}
+// The product's 8-point solve, calib_pose::fit_from_normal: F from the 45-entry upper triangle of a normal matrix in
+// normalised coordinates and T = {s1, tx1, ty1, s2, tx2, ty2}.  Returns 0 if the eigen problem fails.
+int hc_fit_from_normal(const double* up, const double* T, double* F) { return calib_pose::fit_from_normal(up, T, F) ? 1 : 0; }
 
 void hc_motion_from_essential(const double* E, double* Rs /*[4][9]*/, double* ts /*[4][3]*/) {
     double R4[4][9], t4[4][3];

@@ -1,7 +1,7 @@
 """The calibration's device kernels against their host model (tests/calib_util.py), stage by stage, through the public
 entry points: RANSAC (ctx.fundamental_ransac: k_ransac_hypotheses / k_ransac_score / k_ransac_mask), the adjacent
-chain (calibrate_init(method="8point" | "ransac"): k_epipolar_normal, k_sampson_inliers, k_cheirality) and the pose
-graph (calibrate_init(method="graph"): k_epipolar_normal_pairs, k_sampson_pairs, k_pair_cheirality,
+chain (calibrate_init(method="8point" | "ransac"): k_epipolar_normal_pairs, k_sampson_pairs, k_cheirality) and the
+pose graph (calibrate_init(method="graph"): k_epipolar_normal_pairs, k_sampson_pairs, k_pair_cheirality,
 k_translation_normal / k_translation_reduce / k_translation_residuals).  The end-quality bars of
 test_gpu_calib_ransac.py and test_gpu_calib_graph.py cannot see a kernel that drops a ragged tile, a partial sum or a
 point at a tile boundary -- the optimiser absorbs it -- so these compare decisions exactly and values to 1e-9.
@@ -147,6 +147,32 @@ def test_chain_equals_model(torch, libs, method, C, n, frac, seed):
     for c in range(C):
         assert close(poses[c]["R"], model["R"][c], REL), c
         assert np.abs(poses[c]["t"] - model["t"][c]).max() <= REL * max(1.0, np.abs(model["t"][c]).max()), c
+
+
+@pytest.mark.parametrize("method", ["8point", "ransac"])
+def test_chain_is_reproducible(torch, method):
+    """Two calls of calibrate_init(method) on the same tracks return the same bits: F_used, votes, the Sampson sets and
+    the poses.  The re-fits' normal matrices and selections are summed in a fixed order, so nothing depends on the
+    order in which threads finish."""
+    C = 16
+    obs, mask, _, _, _, K, _ = contaminated_tracks(C, 301, 0.2, 36)
+    ctx = _ctx(C, K)
+    a, b = (ctx.calibrate_init(obs, mask, method=method, hypotheses=1000, seed=36) for _ in range(2))
+    for x, y in zip(a[1:], b[1:]):
+        assert np.array_equal(x, y)
+    for p, q in zip(a[0], b[0]):
+        assert np.array_equal(p["R"], q["R"]) and np.array_equal(p["t"], q["t"])
+
+
+def test_chain_launches_do_not_grow_per_pair(torch):
+    """calibrate_init(method="8point"): at most three fit and two Sampson launches for all pairs, then one cheirality
+    launch per pair, at 4 and 16 cameras."""
+    for C, n, seed in ((4, 203, 35), (16, 301, 36)):
+        obs, mask, _, _, _, K, _ = contaminated_tracks(C, n, 0.2, seed)
+        ctx = _ctx(C, K)
+        n0 = ctx.launch_count()
+        ctx.calibrate_init(obs, mask, method="8point")
+        assert ctx.launch_count() - n0 <= 5 + (C - 1), C
 
 
 # ------------------------------------------------------------------------------------------------------------ graph
